@@ -1,10 +1,15 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the sprs product path on B200.
+"""bench.py -- headline benchmark of the sprs product path on H100.
 
 Metric (BASELINE.json): CSR SpMV f64 GFLOP/s and achieved fraction of the HBM roofline
-(2*nnz flops over 12*nnz + 8*n bytes), at 1/2/4/8 B200, beside the sprs CPU path.
+(2*nnz flops over 12*nnz + 8*n bytes), at 1/2/4/8 H100, beside the sprs CPU path.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl reference]
+                  [--dump-outputs DIR]
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy
+(float64; a fixed, seeded sample of rows when the whole result exceeds 64 MB), so that two builds
+can be compared output for output: the inputs are seeded and identical from run to run.
 
 A "step" is one `y = A x` over the whole matrix (all ranks together).  The default
 workload is BASELINE config 5 -- the configuration the metric is quoted on: 10M x 10M
@@ -51,7 +56,29 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f), "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0}, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
+
+
+DUMP_BUDGET = 60_000_000  # bytes of array data --dump-outputs writes, all files together
+DUMP_SEED = 0x5EED0D0
+
+
+def dump_rows(out_dir, name, t, budget=DUMP_BUDGET):
+    """Write a device or host array `t` (1-D, or 2-D row-major) to out_dir/<name>.npy in float64:
+    all of it when it fits `budget` bytes, else a fixed, seeded sample of its rows, with the
+    sampled row numbers (as float64) in <name>_rows.npy."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    rows = t.shape[0]
+    row_bytes = 8 * (t[0].numel() if rows and t.dim() > 1 else 1)
+    if rows * row_bytes <= budget:
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().cpu().numpy().astype(np.float64))
+        return
+    k = budget // (row_bytes + 8)
+    sel = np.sort(np.random.default_rng(DUMP_SEED).choice(rows, size=k, replace=False))
+    idx = torch.from_numpy(sel).to(t.device)
+    np.save(os.path.join(out_dir, name + ".npy"), t[idx].cpu().numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, name + "_rows.npy"), sel.astype(np.float64))
 
 
 class ClockSampler:
@@ -328,6 +355,8 @@ def main():
                          "'nccl' = one NCCL all_gather; 'auto' = the measured default (DESIGN.md 5)")
     ap.add_argument("--no-multicast", action="store_true",
                     help="keep the symmetric buffers on CUDA IPC peer mappings")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's result to DIR/<name>.npy")
     ap.add_argument("--gen-to", default=None, help=argparse.SUPPRESS)
     ap.add_argument("--extra-only", default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -409,8 +438,8 @@ def main():
             cpu_base = {"error": repr(e)}
     t_gen = time.time() - t_gen
     if args.exchange == "auto":
-        # measured at 2 and 8 GPUs (profiles/r2_scale_modes_*.txt; DESIGN.md section 5): the
-        # SpMV kernel storing every finished row itself beats the put kernel and NCCL
+        # the SpMV kernel storing every finished row itself (DESIGN.md section 5;
+        # tools/scale_modes.py times every mode)
         args.exchange = "fused"
     use_comm = world > 1 and args.exchange in ("fused", "push")
 
@@ -546,6 +575,8 @@ def main():
     launches = ctx.launches - launches0
     if comm is not None:
         comm.check()
+    if args.dump_outputs and rank == 0:
+        dump_rows(args.dump_outputs, "y", op.y)  # the whole y = A x of the last timed step
     total_ms = e_start.elapsed_time(e_stop)
     kern_ms = [evs[i][0].elapsed_time(evs[i][1]) for i in range(args.steps)]
     coll_ms = [evs[i][1].elapsed_time(evs[i][2]) for i in range(args.steps)]
@@ -637,9 +668,8 @@ def main():
             try:
                 res = None
                 if name == "spmv_rand_1m":
-                    # a 0.19 ms kernel is the one entry that is sensitive to what the process did
-                    # before it (0.217 ms behind the config-5 legs, 0.186 ms in a process of its
-                    # own, profiles/r2_l2_state_probe.txt): measured in a child process, like
+                    # a sub-millisecond kernel is the one entry that is sensitive to what the
+                    # process did before it: measured in a child process, like
                     # tools/sweep_spmv.py does; in this process only if the child fails
                     res = run_extra_in_child(name)
                 extra[name] = res if res is not None else fn(ctx, G, hbm_peak, dev)
@@ -688,7 +718,7 @@ def main():
                                         "sprs_b200_comm (C ABI: shm rendezvous, %s symmetric buffers, "
                                         "device flag barrier); torch.distributed only broadcasts the id"
                                         % ("VMM + NVSwitch multicast" if multicast else "CUDA IPC")),
-                       "l2_policy": "inputs (%.1f GB) exceed L2 (126 MB); no flush needed" %
+                       "l2_policy": "inputs (%.1f GB) exceed the H100's L2 (50 MB); no flush needed" %
                                     (alg_bytes / 1e9),
                        "gen_seconds": round(t_gen, 1)},
             "achieved_hbm_frac": (alg_bytes / (ms_per_step * 1e-3) / 1e9) / (hbm_peak * world),

@@ -1,7 +1,7 @@
 """bench.py legs for the non-headline workloads of BASELINE.json:
   spmm_rand_1m_k64  (config 3)  CSR x dense C-order 1M x 64  -> csr_mulacc_dense_rowmaj
   spgemm_rmat_500k  (config 4)  two 500k x 500k R-MAT, ~16 nnz/row -> smmp::mul_csr_csr
-Single GPU (the BASELINE configs are single-B200); same JSON contract as bench.py."""
+Single GPU (the BASELINE configs are single-GPU); same JSON contract as bench.py."""
 import ctypes as C
 import json
 import os
@@ -65,6 +65,33 @@ def _cpu_spgemm(A, B, rows):
             "(Automatic: min(rows, (nnzA+nnzB)/8128, ncpu)), 1 run" % (r1, nprod, len(cind))}
 
 
+def dump_csr_rows(out_dir, ctx, cm, rows, dev, budget, seed):
+    """--dump-outputs of the SpGEMM leg: whole rows of the product mirror `cm`, a fixed, seeded
+    sample of them within `budget` bytes, in row order, as float64 arrays c_rows (row numbers),
+    c_indptr (offsets into the sample) and c_indices / c_data (the rows' entries)."""
+    import types
+    import torch
+    import bench as B
+    from sprs_b200 import generate as G
+    d_ip, d_ind, d_dat, ipb = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int()
+    ctx.check(ctx.lib.sprs_b200_csmat_device_arrays(cm, C.byref(d_ip), C.byref(ipb), C.byref(d_ind),
+                                                    C.byref(d_dat)))
+    ip = torch.as_tensor(G._DevArray(d_ip.value, rows + 1, "<i4" if ipb.value == 4 else "<i8"),
+                         device=dev)
+    nnz = G.u32(ip[-1]) if ipb.value == 4 else int(ip[-1].item())
+    c = types.SimpleNamespace(indptr=ip,
+                              indices=torch.as_tensor(G._DevArray(d_ind.value, nnz, "<i4"), device=dev),
+                              data=torch.as_tensor(G._DevArray(d_dat.value, nnz, "<f8"), device=dev))
+    lens = np.diff(ip.cpu().numpy().view(np.uint32 if ipb.value == 4 else np.int64).astype(np.int64))
+    order = np.random.default_rng(seed).permutation(rows)
+    cost = np.cumsum(16 + 16 * lens[order])  # row number + offset, index + value per entry
+    sel = np.sort(order[:int(np.searchsorted(cost, budget, side="right"))])
+    sub_ip, ind, dat = B.rows_to_host(c, torch.from_numpy(sel).to(dev))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in (("c_rows", sel), ("c_indptr", sub_ip), ("c_indices", ind), ("c_data", dat)):
+        np.save(os.path.join(out_dir, name + ".npy"), arr.astype(np.float64))
+
+
 def run(args, ctx, kind, n, npr, gen, seed):
     import torch
     from sprs_b200 import generate as G
@@ -93,6 +120,8 @@ def run(args, ctx, kind, n, npr, gen, seed):
         torch.cuda.synchronize()
         clocks = sampler.stop(tw0, time.time())
         ms = e0.elapsed_time(e1) / args.steps
+        if args.dump_outputs:
+            B.dump_rows(args.dump_outputs, "c", c)
         flops = 2.0 * a.nnz * k
         comp_bytes = 12.0 * a.nnz + 8.0 * k * (n + n)
         # e2e: host B (pinned) in, host C out through the reference-facing call
@@ -131,13 +160,15 @@ def run(args, ctx, kind, n, npr, gen, seed):
     Bm = G.rmat_csr(ctx, n, npr, seed=seed ^ 0x1000)
     lib = ctx.lib
 
-    def once(keep=False):
+    def once(keep=False, keep_c=False):
         plan, nnz_c, cm = C.c_void_p(), C.c_uint64(), C.c_void_p()
         ctx.check(lib.sprs_b200_spgemm_symbolic(ctx.h, A.mirror.h, Bm.mirror.h, C.byref(plan),
                                                 C.byref(nnz_c)))
         ctx.check(lib.sprs_b200_spgemm_numeric_dev(ctx.h, plan, C.byref(cm)))
         nprod = lib.sprs_b200_spgemm_nprod(plan) if keep else 0
         lib.sprs_b200_spgemm_free(plan)
+        if keep_c:
+            return nnz_c.value, cm
         lib.sprs_b200_csmat_free(cm)
         return nnz_c.value, nprod
     nnz_c, nprod = once(keep=True)
@@ -147,11 +178,16 @@ def run(args, ctx, kind, n, npr, gen, seed):
     l0 = ctx.launches
     tw0 = time.time()
     t0 = time.perf_counter()
-    steps = max(3, min(args.steps, 10))
-    for _ in range(steps):
-        once()  # the C-ABI calls are synchronous (they return nnz / a finished mirror)
+    steps = args.steps
+    for i in range(steps):
+        # the C-ABI calls are synchronous (they return nnz / a finished mirror); the last
+        # product is kept for --dump-outputs
+        last = once(keep_c=bool(args.dump_outputs) and i == steps - 1)
     ms = (time.perf_counter() - t0) * 1e3 / steps
     clocks = sampler.stop(tw0, time.time())
+    if args.dump_outputs:
+        dump_csr_rows(args.dump_outputs, ctx, last[1], n, dev, B.DUMP_BUDGET, B.DUMP_SEED)
+        lib.sprs_b200_csmat_free(last[1])
     alg = 12.0 * (A.nnz + nprod + nnz_c) + 8.0 * (n + 1)
     line = {"metric": "csr_spgemm_f64_gflops", "value": 2.0 * nprod / ms / 1e6, "unit": "GFLOP/s",
             "n_gpus": 1, "steps": steps, "warmup": warm, "ms_per_step": ms,

@@ -1,4 +1,4 @@
-/* sprs_b200.h -- C ABI of the B200-native sprs product path.
+/* sprs_b200.h -- C ABI of the H100-native sprs product path.
  *
  * This is the drop-in boundary: exactly what a Rust `sprs-b200-sys` crate would
  * bind (INTEGRATION.md shows the extern "C" block and the safe wrapper).  It

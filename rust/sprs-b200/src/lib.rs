@@ -19,7 +19,7 @@ use std::ffi::CStr;
 use std::ops::Mul;
 use std::os::raw::c_void;
 
-thread_local! { static CTX: Ctx = Ctx::new(0).expect("no B200 device"); }
+thread_local! { static CTX: Ctx = Ctx::new(0).expect("no H100 device"); }
 
 struct Ctx(*mut ffi::sprs_b200_ctx);
 impl Ctx {

@@ -1,4 +1,4 @@
-"""sprs_b200 -- B200-native (sm_100a) implementation of the sprs sparse-product hot
+"""sprs_b200 -- H100-native (sm_90a) implementation of the sprs sparse-product hot
 path (SpMV / SpMM / SpGEMM) behind sprs's operator API.  See DESIGN.md.
 
 Nothing here computes on the CPU: every product is a call into libsprs_b200.so

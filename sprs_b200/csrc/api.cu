@@ -216,8 +216,9 @@ int sprs_b200_ctx_create(int device, sprs_b200_ctx** out) {
         delete ctx;
         return SPRS_B200_ERR_CUDA;
     }
-    if (prop.major < 10) {
-        g_create_error = "sprs_b200 kernels are built for sm_100a only; device is sm_" +
+    // architecture-specific sm_90a code loads on compute capability 9.0 only
+    if (prop.major != 9 || prop.minor != 0) {
+        g_create_error = "sprs_b200 kernels are built for sm_90a (H100) only; device is sm_" +
                          std::to_string(prop.major) + std::to_string(prop.minor);
         cudaStreamDestroy(ctx->stream);
         delete ctx;
@@ -244,7 +245,7 @@ int sprs_b200_ctx_create(int device, sprs_b200_ctx** out) {
         ctx->pol_evict_last = h_pol[1];
     }
     {   // the stream-ordered allocator keeps what the SpGEMM frees (a 42 GB product is
-        // re-allocated by the next call: cudaMalloc / cudaFree of it cost ~100 ms per product)
+        // re-allocated by the next call instead of being mapped again)
         cudaMemPool_t pool;
         if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
             uint64_t keep = ~0ull;

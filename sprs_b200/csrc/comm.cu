@@ -739,7 +739,7 @@ int sprs_b200_spmv_rowpart(sprs_b200_comm* c, const sprs_b200_csmat* mat, const 
     const bool mc = y->mc_ptr != nullptr;
     const bool no_barrier = (exchange & SPRS_B200_EXCHANGE_NO_BARRIER) != 0;
     exchange &= ~SPRS_B200_EXCHANGE_NO_BARRIER;
-    if (exchange == SPRS_B200_EXCHANGE_AUTO)  // measured at 2 and 8 GPUs (profiles/r2_scale_modes_*)
+    if (exchange == SPRS_B200_EXCHANGE_AUTO)  // tools/scale_modes.py times every mode
         exchange = SPRS_B200_EXCHANGE_FUSED;
     SpmvTargets yt;
     yt.n = 1;

@@ -1,4 +1,4 @@
-// common.cuh -- internal types shared by the sm_100a kernels and the C ABI.
+// common.cuh -- internal types shared by the sm_90a kernels and the C ABI.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -11,13 +11,13 @@
 #include "../../include/sprs_b200.h"
 
 constexpr int SPRS_E2E_MAX_CHUNKS = 8;
-constexpr int SPRS_E2E_DEFAULT_CHUNKS = 8;  // host path: y leaves in 8 chunks behind the SpMV (measured
-                                            // 6.86 -> 6.50 ms on config 5; 1 = one launch + one copy)
+constexpr int SPRS_E2E_DEFAULT_CHUNKS = 8;  // host path: y leaves in 8 chunks behind the SpMV
+                                            // (1 = one launch + one copy)
 
 // ---- error plumbing: C functions return int, never throw/abort (SURVEY 8b) ----
 struct sprs_b200_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     size_t l2_bytes = 0;
     cudaStream_t stream = nullptr;  // private stream of the host-buffer entry points
     std::string last_error;

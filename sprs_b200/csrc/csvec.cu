@@ -1,4 +1,4 @@
-// csvec.cu -- CSR matrix x SPARSE vector for sm_100a (B200).
+// csvec.cu -- CSR matrix x SPARSE vector for sm_90a (H100).
 //
 // Replaces prod::csr_mul_csvec (sprs/src/sparse/prod.rs:162-184), what `&A * &v` runs for a
 // CSR matrix and a CsVec (sprs/src/sparse/vec.rs:1104-1131) -- the README example and

@@ -9,7 +9,7 @@
 // does at least this work, so its rate on the bench's own matrix is the ceiling the product
 // kernel is held against (bench.py roofline.gather_ceiling; tools/spmv_lab.cu has the whole
 // design space this variant -- "e8 m2 b2": 256-nnz tiles, next tile's indices prefetched, two
-// CTAs of 8 warps per SM -- won, profiles/r2_lab_ceiling_sweep.txt).
+// CTAs of 8 warps per SM -- is the fastest of).
 #include "common.cuh"
 #include "ptx.cuh"
 

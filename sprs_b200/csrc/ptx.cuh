@@ -1,4 +1,4 @@
-// ptx.cuh -- inline-PTX wrappers shared by the sm_100a kernels: L2 cache policies, hinted
+// ptx.cuh -- inline-PTX wrappers shared by the sm_90a kernels: L2 cache policies, hinted
 // global loads, and the 1-D TMA bulk store shared -> global (cp.async.bulk -> SASS UBLKCP).
 // (tests/emu/transform.py swaps this header for tests/emu/cuemu_ptx.h.)
 #pragma once

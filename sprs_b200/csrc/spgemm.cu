@@ -1,4 +1,4 @@
-// spgemm.cu -- CSR x CSR sparse product for sm_100a (B200).
+// spgemm.cu -- CSR x CSR sparse product for sm_90a (H100).
 //
 // Replaces smmp::mul_csr_csr / mul_csr_csr_with_workspace (sprs/src/sparse/smmp.rs:
 // 196-416): the two-phase Bank-Douglas SMMP product behind `&A * &B`
@@ -61,14 +61,13 @@ constexpr int S_SLOTS = 256;
 constexpr uint32_t SYM_M_SLOTS = 16384, NUM_M_SLOTS = 8192;
 constexpr uint64_t BITMAP_SMEM_MAX_COLS = 200ull * 1024 * 8;  // 200 KB of bits
 
-// Routing and kernel shapes measured in round 2 (profiles/r2_spgemm_notes.md): the hash bins
+// Routing and kernel shapes: the hash bins
 // serve only the rows they are cheap for -- with a shared-memory bitmap the symbolic phase sends
 // rows with n_prod > B.cols/256 to the bitmap kernel, the numeric phase rows with
 // nnz(C_i) > 16 * n_panels to the panel kernel; groups of G warps share one B row when the A row
 // is short (half of config 4's large rows have <= 8 A non-zeros); the CTA-per-row kernels run
 // 1024 threads and keep several 32-entry chunks of B in flight per warp: they are bound by the
-// L2 round trip of the B stream, not by the shared-memory atomics (launch list: 1.5 products per
-// clock per SM with one chunk in flight).
+// L2 round trip of the B stream, not by the shared-memory atomics.
 
 // Warps that share one B row in the CTA-per-row kernels: the largest power of two G with
 // G * na <= nwarps (1 when grouping is off or the A row has at least nwarps/2 non-zeros).
@@ -545,9 +544,6 @@ __global__ void __launch_bounds__(PANEL_NT)
             uint32_t grp_taken = 0;  // G > 1: entries of the group's B row this warp consumed
             bool landed = false;
             // two A non-zeros (kk, kk + ngrp) per pass, their chunks interleaved
-            // two A non-zeros (kk, kk + ngrp) per pass, their chunks interleaved.  (Handing the
-            // pairs out dynamically inside a panel measured 21 % SLOWER than this static deal,
-            // profiles/r2_spgemm_notes.md.)
             for (uint32_t kk = grp; kk < na; kk += 2 * ngrp) {
                 const uint32_t kb = kk + ngrp;
                 const bool has_b = kb < na;
@@ -718,9 +714,7 @@ int plan_large(sprs_b200_ctx* ctx, uint64_t cols, uint32_t n_large, bool need_ac
                LargeWorkspace* w, cudaStream_t s) {
     w->words = (uint32_t)((cols + 31) / 32);
     unsigned grid = (unsigned)std::min<uint64_t>(n_large, (uint64_t)ctx->sm_count * 2);
-    if (need_acc) {  // bound the dense slots to ~8 GB
-        // (tried: only as many slots as fit in L2, with 1024-thread CTAs -- 2.8x SLOWER on
-        // config 4, profiles/r1_bench_spgemm_b.json; parallelism matters more than locality)
+    if (need_acc) {  // bound the dense slots to ~8 GB (10 % of an H100's 80 GB)
         const uint64_t per = cols * sizeof(double);
         const uint64_t cap = std::max<uint64_t>(1, (8ull << 30) / std::max<uint64_t>(per, 1));
         grid = (unsigned)std::min<uint64_t>(grid, cap);
@@ -749,10 +743,8 @@ int run_numeric(sprs_b200_ctx* ctx, sprs_b200_spgemm* p, uint32_t* d_cidx, doubl
     // rows with more than 16 entries per column panel are cheaper in the panel kernel (no
     // probing, no sort; fixed cost ~ n_panels) than in the CTA hash map
     // Hash map or panels?  A row costs the panel kernel ~900 instructions per warp and panel
-    // whatever it holds (ncu: 71 G instructions on config 4, half of the stall samples at the
-    // panel barriers), the CTA hash map pays per product plus a bitonic sort of its table.
-    // Measured on config 4 with the cut at 496 / 1024 / 2048 / 4096 entries: 290 / 249 / 318 /
-    // 307 ms for the whole product (profiles/r2_spgemm_notes.md) -> 1024.
+    // whatever it holds, the CTA hash map pays per product plus a bitonic sort of its table:
+    // the cut sits at 1024 entries.
     const uint32_t num_m_max = std::min<uint32_t>(NUM_M_MAX, 1024);
     bin_rows_kernel<uint32_t><<<grid_for(rows), 256, 0, s>>>(p->d_cnt, rows, NUM_S_MAX, num_m_max,
                                                             p->d_lists, p->d_counters, nullptr);

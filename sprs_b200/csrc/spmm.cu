@@ -1,4 +1,4 @@
-// spmm.cu -- CSR x dense row-major matrix for sm_100a (B200).
+// spmm.cu -- CSR x dense row-major matrix for sm_90a (H100).
 //
 // Replaces prod::csr_mulacc_dense_rowmaj (sprs/src/sparse/prod.rs:189-214), the
 // kernel `&A * &B` picks when B has >= 8 columns (sprs/src/sparse/csmat.rs:2009-2018):
@@ -71,11 +71,8 @@ __global__ void __launch_bounds__(SPMM_NT)
 // column PAIRS 2L + 64 q of the panel, a 512-byte B row at k = 64 is ONE 128-bit request per lane,
 // and the B rows of U consecutive non-zeros are in flight before the first product is added (in
 // storage order, so the sums are the same bits).  The scalar kernel above issues one 8-byte
-// load per non-zero and column and waits for it: two requests in flight per warp; it reached
-// 5.0 TB/s of B-row gathers (76 % of HBM, profiles/r1_ncu_spmm_v1.csv), bound by exposed DRAM
-// latency.  (Round 2 measured two other shapes and dropped them: 4 scalar loads in flight,
-// 3.79 ms, and L2-resident 8-column panels of B with A re-streamed per panel, 5.84 ms, against
-// 2.87 ms -- profiles/r2_spmm_notes.md.)
+// load per non-zero and column and waits for it: two requests in flight per warp, bound by
+// exposed DRAM latency.
 template <typename P, int KV2, int U>
 __global__ void __launch_bounds__(SPMM_NT)
     spmm_rowmaj_vec_kernel(const P* __restrict__ indptr, const uint32_t* __restrict__ indices,

@@ -1,19 +1,18 @@
-// spmv.cu -- CSR x dense-vector product for sm_100a (B200).
+// spmv.cu -- CSR x dense-vector product for sm_90a (H100).
 //
 // Replaces prod::mul_acc_mat_vec_csr (sprs/src/sparse/prod.rs:103-127) and the
 // one-column case of prod::csr_mulacc_dense_colmaj (prod.rs:274-298), which is what
 // `&A * &x` runs (sprs/src/sparse/csmat.rs:2142-2148).
 //
-// Design (DESIGN.md 4.1; evidence in profiles/r2_spmv_notes.md).  The kernel is bound by the x
-// gathers -- the L1TEX pipe, the L1 lines in-flight gathers hold, and the 42 GB they pull through
-// L2 for 12 GB of matrix -- not by HBM: "ceiling" kernels (the same streams and gathers with the
-// row logic removed; tools/spmv_lab.cu, csrc/diag.cu) plateau at 0.55-0.57 of the HBM roofline on
-// the 10M R-MAT and 0.45 on uniform columns whatever the staging.  So:
+// Design (DESIGN.md 4.1).  The kernel is bound by the x gathers -- the L1TEX pipe, the L1 lines
+// in-flight gathers hold, and the 32-byte sector each 8-byte x element pulls through L2 -- not by
+// HBM: "ceiling" kernels (the same streams and gathers with the row logic removed;
+// tools/spmv_lab.cu, csrc/diag.cu) stay well below the HBM roofline whatever the staging.  So:
 //   * MERGE-PATH TILES: the CSR stream is cut where  nnz + 16 * (row ends)  reaches multiples of
 //     1024 (tile_cut_kernel): a tile is ~900 non-zeros of long rows or at most 64 row ends of
 //     empty ones, never a thousand rows for one warp.  A tile belongs to ONE WARP; warps are
 //     persistent and autonomous (no CTA-wide barrier, no shared memory: the whole unified array
-//     is L1 for the gathers -- a max-shared carve-out costs 3x);
+//     is L1 for the gathers);
 //   * ROWS STRAIGHT FROM GLOBAL MEMORY, lanes matched to the rows (rows_direct): per block of 31
 //     rows, tiny rows (<= 8 non-zeros) one lane each in storage order -- the reference's bits
 //     --, the others packed G = 4..32 lanes per row with 4 index / value / gather loads in
@@ -30,10 +29,6 @@
 // Rows longer than 8 non-zeros use trees and agree with the reference to rounding (parity gate:
 // |d| <= 1e-6 * sum|terms|, SURVEY 8d).  Arithmetic is MulAcc::mul_acc's (mul_acc.rs:28-30):
 // unfused multiply, then add.
-// What round 2 measured and dropped on the way here (all parity-green): the round-1 TMA ring with
-// register / shared-memory reductions (0.443), two software-pipelined register-stream kernels
-// with in-register segmented reductions (4.85 and 6.31 ms), index prefetch across steps, 6-8
-// loads per lane, equal-nnz tiles (the sparse tail of the matrix ran at 125 Gnnz/s).
 //
 // Algorithmic bytes per nnz: 12 (8 data + 4 index) + 8 per row (y) -- the BASELINE roofline
 // 12*nnz + 8*n; indptr (4 B/row), the tile cuts (16 B per tile) and x gathers are overhead.
@@ -50,8 +45,8 @@ namespace {
 // tile t is the point (tile_row[t], tile_k[t]) with  k + ROW_COST * r = t * W,  r = the rows
 // whose end has been passed, indptr[r] <= k <= indptr[r+1].  Equal-nnz tiles are not enough on an
 // R-MAT matrix: its sparse tail has stretches of thousands of (nearly) empty rows, a 1024-nnz
-// tile there held ~1700 rows -- 55 dependent boundary fetches for one warp while the others
-// waited (ncu on that region: 125 Gnnz/s against 280 on the dense head, half the warps idle).
+// tile there holds ~1700 rows -- 55 dependent boundary fetches for one warp while the others
+// wait.
 // With the row cost in the cut a tile has at most W / ROW_COST row ends.
 constexpr int SPMV_STAGE_ROWS = 66;  // fused all-gather: staged rows per warp tile (64 row ends + parity pad)
 constexpr uint32_t SPMV_ROW_COST = 16;  // default; 2nd field of SPRS_B200_SPMV_VARIANT for tuning runs
@@ -124,11 +119,9 @@ __device__ __forceinline__ void sink_row(const RowSink& k, uint64_t r, double su
 // Rows [r0, r_last] of one warp tile [k0, k1), straight from global memory -- index, value
 // (L1::no_allocate, L2 evict_first) and the x gather (L2 evict_last), U of each in flight per
 // lane; nothing is staged and nothing but a row sum crosses lanes (~1 instruction per non-zero on
-// long rows, against ~1.5 for reducing products staged in shared memory or registers,
-// profiles/r2_spmv_notes.md).  Row boundaries come 31 rows at a time (lane L: indptr[rbase + L]),
-// and every block of 31 rows is taken in three sweeps, because R-MAT blocks mix rows of 0, 5, 50
-// and 5000 non-zeros and any single lanes-per-row choice leaves most lanes idle (ncu on the
-// sparse tail of config 5: 23 of 32 lanes active, 125 Gnnz/s against 280 on the dense head):
+// long rows).  Row boundaries come 31 rows at a time (lane L: indptr[rbase + L]), and every block
+// of 31 rows is taken in three sweeps, because R-MAT blocks mix rows of 0, 5, 50 and 5000
+// non-zeros and any single lanes-per-row choice leaves most lanes idle:
 //   1. TINY rows (at most 2U = 8 non-zeros, empty rows included): every lane takes its own row,
 //      all of them in one pass, summed in storage order -- the reference's bits for every such row;
 //   2. the other rows, packed (no slot is spent on a tiny row): G lanes per row, 32/G rows per
@@ -282,10 +275,8 @@ __global__ void __launch_bounds__(NWARPS * 32, MINB)
     sink.stage = nullptr;
     sink.stage_off = 0;
     // The peers' copies of y (fused all-gather).  A store per finished row and peer slows the
-    // ISSUING kernel in proportion to rows x peers (8 GPUs over IPC mappings,
-    // profiles/r2_scale_modes_8gpu_tma_vs_direct.txt: +0.03 ms on the dense head rank, +0.31 ms
-    // on a tail rank with 3 M rows, against 0.53 ms of compute): remote stores queue in the LSU
-    // in front of the loads.  With stage_rows set, the rows of a tile are staged in shared memory
+    // ISSUING kernel in proportion to rows x peers: remote stores queue in the LSU in front of
+    // the loads.  With stage_rows set, the rows of a tile are staged in shared memory
     // (at most 64 row ends per tile = 512 bytes per warp) and leave through the TMA instead -- one
     // cp.async.bulk per target and tile.  Bulk copies need 16-byte alignment on both
     // sides: row r sits at stage[r + par - even base] with par = the parity of the peers' y
@@ -452,8 +443,8 @@ __global__ void spmv_fixup_range_kernel(const uint32_t* __restrict__ tile_row, c
 // ---- launch configuration ---------------------------------------------------------
 // One kernel configuration ships: 8-warp CTAs, 5 per SM (= __launch_bounds__ minBlocks: the
 // register budget; the kernel hides latency with warps, not registers), 4 loads of each kind in
-// flight per lane.  Round 2 swept 4-6 CTAs/SM and 4 / 6 / 8 loads (profiles/r2_spmv_notes.md):
-// the others lost and were deleted.  The two numbers of the CUT stay tunable for experiments:
+// flight per lane (48 registers on sm_90a, no spills).  The two numbers of the CUT stay tunable
+// for experiments:
 // SPRS_B200_SPMV_VARIANT="w,row_cost" (cost units per tile, cost of a row end in non-zeros;
 // read once per process -- they are baked into every mirror's tile arrays).
 struct SpmvVariant {
@@ -488,7 +479,7 @@ int launch_variant(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const double* d
     bool& configured = configured_flags[ctx->device & 63][multi ? 1 : 0];
     if (!configured) {
         // no shared memory at all: the whole unified array is L1 for the gathers (every
-        // in-flight gather holds an L1 line; lab carve sweep: 0 % 303, 50 % 275, 100 % 106 Gnnz/s)
+        // in-flight gather holds an L1 line)
         // (the multi-target kernel stages 4.1 KB per CTA for its TMA stores: 5 CTAs need 26 KB)
         int carve = multi ? 15 : 0;
         if (const char* e = getenv("SPRS_B200_SPMV_CARVEOUT")) carve = atoi(e);
@@ -496,11 +487,11 @@ int launch_variant(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const double* d
                                             carve));
         configured = true;
     }
-    // How the peers get their rows (8 GPUs, profiles/r2_scale_modes_8gpu_tma_vs_direct.txt):
+    // How the peers get their rows:
     //   * several peer mappings (CUDA IPC / VMM, world-1 targets): staged per tile and sent by
-    //     TMA bulk stores -- 0.718 ms per step against 0.862 with a store per row and target;
-    //   * ONE multicast target: a plain store per row -- 0.601 against 0.639 staged (one store
-    //     per row is cheap enough, and the staged form waits on the TMA between tiles).
+    //     TMA bulk stores instead of a store per row and target;
+    //   * ONE multicast target: a plain store per row (one store per row is cheap enough, and
+    //     the staged form waits on the TMA between tiles).
     // Staging also needs all targets to agree on the 16-byte parity of their address.
     // SPRS_B200_SPMV_PEER_STORES=direct|tma forces one form (read per launch:
     // tools/scale_modes.py times both).

@@ -93,6 +93,11 @@ def _keys_to_csr(ctx, keys, rows, cols, seed):
         ctx.check(lib.sprs_b200_gen_normal_from_keys(ctx.h, seed ^ 0xDA7A, _dptr(keys), n,
                                                      _dptr(data), _stream_ptr()))
     _sync()
+    if dev.type == "cuda":
+        # the sorts above leave several times the matrix in torch's cache (tens of GB for the
+        # 1e9-nnz R-MAT); the library allocates outside that cache (cudaMalloc, its
+        # stream-ordered pool), so on an 80 GB H100 it is handed back before the matrix is used
+        torch.cuda.empty_cache()
     return DeviceCsr(ctx, rows, cols, indptr, indices, data)
 
 

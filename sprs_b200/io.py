@@ -87,7 +87,7 @@ class TriMat:
         """TriMat::to_csr (triplet_iter.rs:115-124) on the device."""
         from .sparse import CsMat
         if self.dtype != np.float64:
-            raise TypeError("the B200 path is f64 only; %s triplets stay on the host" % self.dtype)
+            raise TypeError("the H100 path is f64 only; %s triplets stay on the host" % self.dtype)
         return CsMat.from_triplets(self.shape, self.row_inds, self.col_inds, self.data, ctx=ctx)
 
     def to_csc(self, ctx=None):

@@ -539,7 +539,7 @@ class prod:
     @staticmethod
     def _dense(name, lhs, rhs, out):
         if rhs.dtype != np.float64 or out.dtype != np.float64:
-            raise TypeError("f64 only on the B200 path (other N stay on the CPU code)")
+            raise TypeError("f64 only on the H100 path (other N stay on the CPU code)")
         # assert order of prod.rs:198-201
         if lhs.cols() != rhs.shape[0] or lhs.rows() != out.shape[0] or \
                 rhs.shape[1] != out.shape[1]:

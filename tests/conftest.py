@@ -23,7 +23,7 @@ def emu_library():
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
     if os.environ.get("SPRS_B200_EMU") == "1":
         # developer switch: run `-m gpu` tests against the emulator (those that only need the
         # C ABI and numpy work; the ones that allocate through torch.cuda do not)

@@ -387,7 +387,7 @@ cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
     p->multiProcessorCount = 4;  // small grids keep the emulation quick
     p->l2CacheSize = 1 << 20;
     p->totalGlobalMem = (size_t)1 << 32;
-    p->major = 10;
+    p->major = 9;  // the compute capability the library is built for (sm_90a)
     p->minor = 0;
     return cudaSuccess;
 }

@@ -5,7 +5,7 @@ The library's own sources are compiled for the CPU, unmodified apart from a mech
 rewrite of launches / shared-memory declarations / the PTX wrappers, into a SEPARATE library
 that only this file and `SPRS_B200_EMU=1 pytest -m gpu` load.  This finds indexing, barrier
 and host-sequencing bugs where no GPU is attached; it is NOT parity evidence (that is the
-`-m gpu` suite on the B200) and says nothing about performance or the hardware memory model.
+`-m gpu` suite on the H100) and says nothing about performance or the hardware memory model.
 """
 import os
 import subprocess

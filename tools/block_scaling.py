@@ -1,7 +1,5 @@
 """Row blocks of 1/8 .. 1 of the config-5 matrix (full x) on one GPU: how the SpMV rate depends
-on the block (rows per non-zero differ 3x between the head and the tail of an R-MAT matrix).
-(Round 2 also tried a persisting-L2 access-policy window for x here: 12 % SLOWER on every block,
-profiles/r2_block_scaling.txt; the kernels' L2::evict_last hints already keep x resident.)"""
+on the block (rows per non-zero differ 3x between the head and the tail of an R-MAT matrix)."""
 import ctypes as C
 import json
 import os

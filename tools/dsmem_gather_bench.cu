@@ -7,9 +7,9 @@
 // Threads stream random indices from global memory (coalesced, 4 B each) and gather table
 // entries with ld.shared::cluster (cluster.map_shared_rank), U loads in flight per thread.
 // Cluster size 1 measures plain shared-memory random reads (bank conflicts only).
-// Prints G elements/s and elements per clock per SM; compare with 1.0/clk/SM for global gathers
-// (profiles/r1_gather_microbench.txt).
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a tools/dsmem_gather_bench.cu -o dsmem_gather_bench
+// Prints G elements/s and elements per clock per SM; compare with tools/gather_bench.cu's global
+// gathers.
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a tools/dsmem_gather_bench.cu -o dsmem_gather_bench
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
@@ -67,7 +67,7 @@ int main() {
     CK(cudaMalloc(&idx, n * 4)); CK(cudaMalloc(&out, 64));
     fill_idx<<<(unsigned)((n + 255) / 256), 256>>>(idx, n, 16u * PER_CTA);
     CK(cudaDeviceSynchronize());
-    int sms = 148, khz = 1965000;
+    int sms = 132, khz = 1980000;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
     auto kern = dsmem_gather_k<8>;

@@ -1,9 +1,9 @@
-// gather_bench.cu -- microbenchmarks that bound the SpMV design on B200 (DESIGN.md):
+// gather_bench.cu -- microbenchmarks that bound the SpMV design on H100 (DESIGN.md):
 //   copy     : streaming read+write bandwidth (the HBM roofline denominator's cousin)
 //   stream   : read-only stream of 12 B/element (index + value), like the CSR arrays
 //   gather   : random 8-byte gathers from a table of T bytes (x of an SpMV)
 //   spmvlike : stream 12 B + 1 random gather per element (no reduction)
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a tools/gather_bench.cu -o gather_bench
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a tools/gather_bench.cu -o gather_bench
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -70,7 +70,7 @@ int main() {
     CK(cudaMalloc(&idx, n * 4)); CK(cudaMalloc(&val, n * 8)); CK(cudaMalloc(&x, 1ull << 30)); CK(cudaMalloc(&out, 64)); CK(cudaMalloc(&cp, n * 8));
     fill_val<<<(unsigned)((n + 255) / 256), 256>>>(val, n);
     fill_val<<<(unsigned)(((1ull << 27) + 255) / 256), 256>>>(x, 1ull << 27);
-    int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     float ms = timeit([&] { copy_k<<<sms * 16, 512>>>((const double4*)val, (double4*)cp, n / 4); });
     printf("copy      : %.3f ms  %.1f GB/s (read+write)\n", ms, 2.0 * n * 8 / ms / 1e6);
     ms = timeit([&] { stream_k<<<sms * 16, 512>>>(idx, val, out, n); });

@@ -5,8 +5,7 @@ a,b,c,d = .57,.19,.19,.05, scale 24, n = 1e7, ~100 nnz/row), walks the non-zeros
 SpMV kernel does (32 consecutive non-zeros per warp gather instruction) and counts, per
 non-zero, the distinct 128-byte lines (L1TEX wavefronts) and 32-byte sectors (L2->SM traffic)
 the x gathers touch -- with and without a cache of the K most frequent columns.
-The no-cache figures can be checked against ncu (profiles/r1_ncu_spmv_v4_*: 0.66 lines and
-0.94 sectors per non-zero).
+The no-cache figures can be checked against ncu's L1TEX / L2 sector counts of the SpMV kernel.
 """
 import sys
 

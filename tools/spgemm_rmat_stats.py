@@ -2,8 +2,7 @@
 16 nnz/row, C = A * B -- to see where the SpGEMM's products are: by nnz(C_i), by the length of
 the A row and of the B rows streamed, and how full the 32-lane chunks of the column-panel
 kernel are.  numpy regeneration of the same distribution (not the same seed as csrc/gen.cu).
-Output kept in profiles/r1_spgemm_rmat_stats.txt; it is the evidence behind the
-SPRS_B200_SPGEMM_V2 routing in csrc/spgemm.cu."""
+It is the evidence behind the row routing in csrc/spgemm.cu."""
 import numpy as np, sys
 rng = np.random.default_rng(4)
 SCALE, N, NPR = 19, 500_000, 16

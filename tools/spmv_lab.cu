@@ -1,4 +1,4 @@
-// spmv_lab.cu -- design-space probe for the SpMV gather pipe on B200 (NOT product code).
+// spmv_lab.cu -- design-space probe for the SpMV gather pipe on H100 (NOT product code).
 //
 // "Ceiling" kernels: the SpMV's memory behaviour with the row logic removed -- stream the
 // (index, value) arrays of a REAL matrix in warp tiles, gather x[col], multiply-add into one
@@ -17,7 +17,7 @@
 //   MINB  resident CTAs per SM (8 warps each) -- sets the register budget
 // cmode: 0 real columns, 1 columns & mask (shrinks the x range), 2 sequential columns.
 //
-// Build: make -C tools lab   (nvcc -shared, sm_100a)
+// Build: make -C tools lab   (nvcc -shared, sm_90a)
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -217,7 +217,7 @@ int run(const uint32_t* idx, const double* val, const double* x, double* out, ui
 extern "C" int lab_ceiling(int epl, int mode, int gop, int minb, int carve_pct, int cmode,
                            uint32_t mask, uint32_t ncols, const uint32_t* idx, const double* val,
                            const double* x, double* out, uint64_t nnz, int iters, float* ms) {
-    int dev = 0, sm = 148;
+    int dev = 0, sm = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, dev);
 #define CASE(E, M, G, B)                                                                     \
