@@ -421,6 +421,8 @@ int sprs_b200_csmat_free(sprs_b200_csmat* m) {
     if (m->d_tile_row) cudaFree(m->d_tile_row);
     if (m->d_tile_k) cudaFree(m->d_tile_k);
     if (m->d_carry) cudaFree(m->d_carry);
+    if (m->d_hot_col) cudaFree(m->d_hot_col);
+    if (m->d_hot_idx) cudaFree(m->d_hot_idx);
     if (m->csr_cache) sprs_b200_csmat_free(m->csr_cache);
     delete m;
     return SPRS_B200_OK;

@@ -57,6 +57,12 @@ struct sprs_b200_csmat {
     void* d_tile_k = nullptr;      // nnz position of every cut (as wide as the indptr)
     double* d_carry = nullptr;
     uint64_t n_tiles = 0;
+    // SpMV hot set (spmv.cu, DESIGN.md 4.1): the n_hot most-referenced columns (hot_col, K
+    // entries) and the index stream the SpMV reads instead of d_indices, each hot column tagged
+    // as 0x80000000 | slot (hot_idx, nnz entries: +4 bytes per non-zero).  n_hot == 0: none.
+    uint32_t* d_hot_col = nullptr;
+    uint32_t* d_hot_idx = nullptr;
+    uint32_t n_hot = 0;
     // CSC mirrors only: the CSR conversion the product kernels run on, built on first use
     // by the host-buffer entry points and kept until the mirror is freed.
     mutable sprs_b200_csmat* csr_cache = nullptr;
@@ -111,7 +117,8 @@ struct SpmvTargets {
 };
 
 // ---- kernels' launch wrappers (defined in the .cu files) -----------------------
-int spmv_prepare(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s);
+// SpMV side arrays of a CSR mirror: the tile cuts, and (hot_set) the hot set where it pays
+int spmv_prepare(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, bool hot_set = true);
 int spmv_tile_nnz();  // non-zeros per SpMV warp tile (fixed per process)
 int spmv_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const double* d_x, double* d_y,
                 int accumulate, cudaStream_t s);

@@ -961,7 +961,9 @@ int sprs_b200_spgemm_numeric_dev(sprs_b200_ctx* ctx, sprs_b200_spgemm* p, sprs_b
             cudaMemcpyAsync(m->d_indptr, p->d_cptr, (m->rows + 1) * 8, cudaMemcpyDeviceToDevice, s);
         }
         if ((st = run_numeric(ctx, p, m->d_indices, m->d_data, s)) != SPRS_B200_OK) break;
-        if ((st = spmv_prepare(ctx, m, s)) != SPRS_B200_OK) break;
+        // (no SpMV hot set for a product: its build would run inside every SpGEMM call and
+        // would need 4 more bytes per non-zero next to a result that may fill the device)
+        if ((st = spmv_prepare(ctx, m, s, false)) != SPRS_B200_OK) break;
         if (cudaStreamSynchronize(s) != cudaSuccess || cudaGetLastError() != cudaSuccess) {
             sprs_b200_set_error(ctx, "spgemm numeric: kernel failed");
             st = SPRS_B200_ERR_CUDA;

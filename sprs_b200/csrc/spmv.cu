@@ -25,7 +25,10 @@
 //   * the multi-target flavour (fused all-gather of the multi-GPU path, DESIGN.md 5) also
 //     delivers every finished row to the peers: a plain store into ONE multicast address, or --
 //     several peer mappings -- the tile's rows staged in 528 bytes of shared memory per warp and
-//     sent as one TMA bulk store per peer (the only shared memory in this file).
+//     sent as one TMA bulk store per peer;
+//   * HOT SET (large skewed matrices, spmv_prepare_hot): x of the K most-referenced columns is
+//     staged in shared memory by every CTA (one 32-warp CTA per SM) and the kernel reads a
+//     tagged copy of the index stream, so those gathers move no L2 sector.
 // Rows longer than 8 non-zeros use trees and agree with the reference to rounding (parity gate:
 // |d| <= 1e-6 * sum|terms|, SURVEY 8d).  Arithmetic is MulAcc::mul_acc's (mul_acc.rs:28-30):
 // unfused multiply, then add.
@@ -35,7 +38,9 @@
 
 #include "common.cuh"
 #include "ptx.cuh"
+#include "scan.cuh"
 
+#include <algorithm>
 #include <cstdlib>
 
 namespace {
@@ -116,6 +121,18 @@ __device__ __forceinline__ void sink_row(const RowSink& k, uint64_t r, double su
     }
 }
 
+// x[c] for an entry of the index stream.  On a mirror with a hot set the SpMV reads the TAGGED
+// copy of the stream: a hot column is stored as HOT_TAG | slot and its x value comes from the
+// CTA's shared-memory copy of the hot set instead of a gathered L2 sector.  The value is the
+// same double either way, so every product and sum keeps its bits.
+constexpr uint32_t HOT_TAG = 0x80000000u;
+template <bool HOT>
+__device__ __forceinline__ double gather_x(const double* __restrict__ x, const double* hot,
+                                           uint32_t c, uint64_t polx) {
+    if (HOT && (c & HOT_TAG)) return hot[c & ~HOT_TAG];
+    return ldg_f64_hint(x + c, polx);
+}
+
 // Rows [r0, r_last] of one warp tile [k0, k1), straight from global memory -- index, value
 // (L1::no_allocate, L2 evict_first) and the x gather (L2 evict_last), U of each in flight per
 // lane; nothing is staged and nothing but a row sum crosses lanes (~1 instruction per non-zero on
@@ -127,11 +144,11 @@ __device__ __forceinline__ void sink_row(const RowSink& k, uint64_t r, double su
 //   2. the other rows, packed (no slot is spent on a tiny row): G lanes per row, 32/G rows per
 //      pass, each group walking its row with stride G; one G-lane butterfly finishes a row;
 //   3. rows longer than 4 steps of their group: the whole warp, one row at a time.
-template <typename P, int G, int U, bool MULTI>
+template <typename P, int G, int U, bool MULTI, bool HOT>
 __device__ __forceinline__ void rows_direct(const RowSink& k, const P* __restrict__ indptr,
                                             const uint32_t* __restrict__ indices,
                                             const double* __restrict__ data,
-                                            const double* __restrict__ x, P k0, P k1,
+                                            const double* __restrict__ x, const double* hot, P k0, P k1,
                                             uint32_t r0, uint32_t r_last, P b_first,
                                             uint64_t pol_stream, uint64_t polx, int lane) {
     constexpr int NG = 32 / G;
@@ -168,7 +185,7 @@ __device__ __forceinline__ void rows_direct(const RowSink& k, const P* __restric
                     v[u] = (tiny && q + (P)u < me) ? ldg_stream_f64(data + q + (P)u, pol_stream) : 0.0;
 #pragma unroll
                 for (int u = 0; u < U; ++u)
-                    xv[u] = (tiny && q + (P)u < me) ? ldg_f64_hint(x + c[u], polx) : 0.0;
+                    xv[u] = (tiny && q + (P)u < me) ? gather_x<HOT>(x, hot, c[u], polx) : 0.0;
 #pragma unroll
                 for (int u = 0; u < U; ++u)
                     if (tiny && q + (P)u < me) acc = __dadd_rn(acc, __dmul_rn(v[u], xv[u]));
@@ -211,7 +228,7 @@ __device__ __forceinline__ void rows_direct(const RowSink& k, const P* __restric
                     v[u] = q + (P)(u * G) < e ? ldg_stream_f64(data + q + (P)(u * G), pol_stream) : 0.0;
 #pragma unroll
                 for (int u = 0; u < U; ++u)
-                    xv[u] = q + (P)(u * G) < e ? ldg_f64_hint(x + c[u], polx) : 0.0;
+                    xv[u] = q + (P)(u * G) < e ? gather_x<HOT>(x, hot, c[u], polx) : 0.0;
 #pragma unroll
                 for (int u = 0; u < U; ++u)
                     if (q + (P)(u * G) < e) acc = __dadd_rn(acc, __dmul_rn(v[u], xv[u]));
@@ -238,7 +255,7 @@ __device__ __forceinline__ void rows_direct(const RowSink& k, const P* __restric
                             v[u] = q + (P)(u * 32) < qe ? ldg_stream_f64(data + q + (P)(u * 32), pol_stream) : 0.0;
 #pragma unroll
                         for (int u = 0; u < U; ++u)
-                            xv[u] = q + (P)(u * 32) < qe ? ldg_f64_hint(x + c[u], polx) : 0.0;
+                            xv[u] = q + (P)(u * 32) < qe ? gather_x<HOT>(x, hot, c[u], polx) : 0.0;
 #pragma unroll
                         for (int u = 0; u < U; ++u)
                             if (q + (P)(u * 32) < qe) a2 = __dadd_rn(a2, __dmul_rn(v[u], xv[u]));
@@ -253,7 +270,7 @@ __device__ __forceinline__ void rows_direct(const RowSink& k, const P* __restric
     }
 }
 
-template <typename P, int NWARPS, int MINB, int U, bool MULTI>
+template <typename P, int NWARPS, int MINB, int U, bool MULTI, bool HOT>
 __global__ void __launch_bounds__(NWARPS * 32, MINB)
     spmv_rows_kernel(const P* __restrict__ indptr, const uint32_t* __restrict__ indices,
                      const double* __restrict__ data, const uint32_t* __restrict__ tile_row,
@@ -262,11 +279,21 @@ __global__ void __launch_bounds__(NWARPS * 32, MINB)
                      double* __restrict__ carry, uint64_t nnz, uint32_t rows, uint32_t t_begin,
                      uint32_t t_end /* this launch covers tiles [t_begin, t_end) */, int accumulate,
                      uint64_t pol_stream /* L2 evict_first */, uint64_t polx /* L2 evict_last */,
-                     int stage_rows /* MULTI: peers get their rows by TMA bulk stores (0: plain stores) */) {
+                     int stage_rows /* MULTI: peers get their rows by TMA bulk stores (0: plain stores) */,
+                     const uint32_t* __restrict__ hot_col /* HOT: the columns of the slots */,
+                     uint32_t n_hot) {
     // (the two L2 policies are kernel PARAMETERS: warp-uniform by construction, so they live in
     // uniform registers; as per-thread createpolicy results every hinted load re-materialised
     // its descriptor)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // HOT: x of the hot columns, one copy per CTA in dynamic shared memory (`indices` is then
+    // the tagged stream)
+    extern __shared__ __align__(16) double hot_x[];
+    if constexpr (HOT) {
+        for (uint32_t q = threadIdx.x; q < n_hot; q += NWARPS * 32)
+            hot_x[q] = ldg_f64_hint(x + hot_col[q], polx);
+        __syncthreads();
+    }
     const uint32_t GW = gridDim.x * NWARPS;
     RowSink sink;
     sink.y = yt.p[0];
@@ -322,8 +349,8 @@ __global__ void __launch_bounds__(NWARPS * 32, MINB)
         const uint32_t r_last = r1 < rows ? r1 : r1 - 1;
         const uint64_t cnt = k1 - k0, nr = (uint64_t)(r_last - r0) + 1;  // mean row length = cnt / nr
 #define SPMV_ROWS(G)                                                                            \
-    rows_direct<P, G, U, MULTI>(sink, indptr, indices, data, x, k0, k1, r0, r_last, b_first,       \
-                             pol_stream, polx, lane)
+    rows_direct<P, G, U, MULTI, HOT>(sink, indptr, indices, data, x, hot_x, k0, k1, r0, r_last,   \
+                                     b_first, pol_stream, polx, lane)
         if (cnt <= 24 * nr)
             SPMV_ROWS(4);
         else if (cnt <= 48 * nr)
@@ -465,24 +492,82 @@ SpmvVariant spmv_variant() {
 
 constexpr int SPMV_NWARPS = 8, SPMV_CTAS_PER_SM = 5, SPMV_LOADS_IN_FLIGHT = 4;
 
+// ---- hot set: the most-referenced columns of x, served from shared memory --------------
+// R-MAT columns are heavily skewed: a few thousand columns take a large share of the non-zeros,
+// but every gather of one of them still moves a 32-byte L2 sector into an L1 that cold gathers
+// keep evicting.  A mirror with a hot set carries the K most-referenced columns (hot_col) and a
+// tagged copy of its index stream for the SpMV (hot_idx: HOT_TAG | slot for a hot column); every
+// CTA stages x of the hot columns in shared memory at kernel start.  The hot-set kernel runs
+// fewer, larger CTAs, because each CTA holds one copy: one 32-warp CTA per SM (64 registers, no
+// spills).  Measured on config 5 (DESIGN.md 4.1): K = 24576 beat 12288 and 16384, and two 20-warp
+// CTAs per SM with 8192 slots each were slower (and spill at their 48-register budget).
+constexpr int SPMV_HOT_NWARPS = 32, SPMV_HOT_CTAS_PER_SM = 1;
+constexpr uint32_t SPMV_HOT_SLOTS = 24576;       // K of `auto` (192 KB of x per CTA)
+constexpr uint32_t SPMV_HOT_MAX_SLOTS = 26624;   // 208 KB + the MULTI stage fit one CTA
+// `auto` builds the hot set only where it pays: enough non-zeros to hide the staging of K
+// values per CTA and launch, and a hot set that serves a real share of them (a uniform matrix
+// like BASELINE config 2 has ~1 %).
+constexpr uint64_t SPMV_HOT_MIN_NNZ = 1ull << 25;
+constexpr double SPMV_HOT_MIN_SHARE = 0.10;
+
+// SPRS_B200_SPMV_HOT=auto|0|K (read once per process): `auto` (default) = K = SPMV_HOT_SLOTS
+// where the thresholds above hold; 0 = never; K = a hot set of K slots on every CSR mirror that
+// can have one (A/B runs and tests).
+struct SpmvHot {
+    uint32_t k;
+    bool forced;
+};
+SpmvHot spmv_hot() {
+    static SpmvHot h = [] {
+        SpmvHot d{SPMV_HOT_SLOTS, false};
+        const char* e = getenv("SPRS_B200_SPMV_HOT");
+        if (e && strcmp(e, "auto") != 0) {
+            const long k = atol(e);
+            d = SpmvHot{(uint32_t)(k < 0 ? 0 : k > (long)SPMV_HOT_MAX_SLOTS ? SPMV_HOT_MAX_SLOTS : k), true};
+        }
+        return d;
+    }();
+    return h;
+}
+
+template <typename P, bool MULTI, bool HOT>
+auto* spmv_kernel() {
+    constexpr int U = SPMV_LOADS_IN_FLIGHT;
+    if constexpr (HOT)
+        return spmv_rows_kernel<P, SPMV_HOT_NWARPS, SPMV_HOT_CTAS_PER_SM, U, MULTI, true>;
+    else
+        return spmv_rows_kernel<P, SPMV_NWARPS, SPMV_CTAS_PER_SM, U, MULTI, false>;
+}
+
 template <typename P>
 int launch_variant(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const double* d_x,
                    const SpmvTargets& yt, int accumulate, uint64_t t0, uint64_t t1,
                    cudaStream_t s) {
     if (m->n_tiles >= 0xffffffffull)
         SPRS_FAIL(ctx, SPRS_B200_ERR_UNSUPPORTED, "spmv: more than 2^32 tiles");
-    constexpr int CTAS = SPMV_CTAS_PER_SM, U = SPMV_LOADS_IN_FLIGHT;
-    const bool multi = yt.n > 1;
-    auto kern = multi ? spmv_rows_kernel<P, SPMV_NWARPS, CTAS, U, true>
-                      : spmv_rows_kernel<P, SPMV_NWARPS, CTAS, U, false>;
-    static bool configured_flags[64][2] = {};  // function attributes are per device
-    bool& configured = configured_flags[ctx->device & 63][multi ? 1 : 0];
+    const bool multi = yt.n > 1, hot = m->n_hot > 0;
+    auto kern = hot ? (multi ? spmv_kernel<P, true, true>() : spmv_kernel<P, false, true>())
+                    : (multi ? spmv_kernel<P, true, false>() : spmv_kernel<P, false, false>());
+    const int nwarps = hot ? SPMV_HOT_NWARPS : SPMV_NWARPS;
+    const int ctas = hot ? SPMV_HOT_CTAS_PER_SM : SPMV_CTAS_PER_SM;
+    static bool configured_flags[64][4] = {};  // function attributes are per device
+    bool& configured = configured_flags[ctx->device & 63][(multi ? 1 : 0) + (hot ? 2 : 0)];
     if (!configured) {
-        // no shared memory at all: the whole unified array is L1 for the gathers (every
-        // in-flight gather holds an L1 line)
-        // (the multi-target kernel stages 4.1 KB per CTA for its TMA stores: 5 CTAs need 26 KB)
-        int carve = multi ? 15 : 0;
-        if (const char* e = getenv("SPRS_B200_SPMV_CARVEOUT")) carve = atoi(e);
+        int carve;
+        if (hot) {
+            // room for the largest hot set this process builds, in every CTA of the SM
+            // (+ the multi-target stage, + the 1 KB the hardware reserves per CTA)
+            const int dyn = (int)(spmv_hot().k * sizeof(double));
+            const int per_cta = dyn + (multi ? nwarps * SPMV_STAGE_ROWS * 8 : 0) + 1024;
+            SPRS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
+            carve = (int)((100ull * ctas * per_cta + 228 * 1024 - 1) / (228 * 1024));
+        } else {
+            // no shared memory at all: the whole unified array is L1 for the gathers (every
+            // in-flight gather holds an L1 line)
+            // (the multi-target kernel stages 4.1 KB per CTA for its TMA stores: 5 CTAs need 26 KB)
+            carve = multi ? 15 : 0;
+            if (const char* e = getenv("SPRS_B200_SPMV_CARVEOUT")) carve = atoi(e);
+        }
         SPRS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
                                             carve));
         configured = true;
@@ -505,16 +590,183 @@ int launch_variant(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const double* d
         for (int q = 2; q < yt.n; ++q)
             if ((((uintptr_t)yt.p[q] ^ (uintptr_t)yt.p[1]) >> 3) & 1) stage_rows = 0;
     }
-    uint64_t grid = (uint64_t)ctx->sm_count * CTAS;
-    const uint64_t need = (t1 - t0 + SPMV_NWARPS - 1) / SPMV_NWARPS;
+    uint64_t grid = (uint64_t)ctx->sm_count * ctas;
+    const uint64_t need = (t1 - t0 + nwarps - 1) / nwarps;
     if (grid > need) grid = need;
-    kern<<<(unsigned)grid, SPMV_NWARPS * 32, 0, s>>>((const P*)m->d_indptr, m->d_indices,
-                                                     m->d_data, m->d_tile_row, (const P*)m->d_tile_k, d_x, yt,
-                                                     m->d_carry,
-                                                     m->nnz, (uint32_t)m->rows, (uint32_t)t0,
-                                                     (uint32_t)t1, accumulate, ctx->pol_evict_first,
-                                                     ctx->pol_evict_last, stage_rows);
+    const size_t smem = hot ? m->n_hot * sizeof(double) : 0;
+    kern<<<(unsigned)grid, nwarps * 32, smem, s>>>((const P*)m->d_indptr,
+                                                   hot ? m->d_hot_idx : m->d_indices,
+                                                   m->d_data, m->d_tile_row, (const P*)m->d_tile_k, d_x, yt,
+                                                   m->d_carry,
+                                                   m->nnz, (uint32_t)m->rows, (uint32_t)t0,
+                                                   (uint32_t)t1, accumulate, ctx->pol_evict_first,
+                                                   ctx->pol_evict_last, stage_rows, m->d_hot_col,
+                                                   m->n_hot);
     return SPRS_B200_OK;
+}
+
+// ---- hot-set construction (spmv_prepare) --------------------------------------------
+// Warp-aggregated increment: the lanes holding the same key add once (the top column of an
+// R-MAT matrix is referenced ~1e6 times).  `active` = the lanes taking part.
+__device__ __forceinline__ void add_aggregated(uint32_t* counts, uint32_t key, unsigned active) {
+    const unsigned peers = __match_any_sync(active, key);
+    if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(counts + key, (uint32_t)__popc(peers));
+}
+
+// counts[c] = references of column c in the index stream
+__global__ void hot_count_kernel(const uint32_t* __restrict__ indices, uint64_t nnz,
+                                 uint32_t* __restrict__ counts) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t base = blockIdx.x * (uint64_t)blockDim.x + (threadIdx.x & ~31u); base < nnz;
+         base += stride) {
+        const uint64_t i = base + (threadIdx.x & 31);
+        const bool valid = i < nnz;
+        const unsigned active = __ballot_sync(0xffffffffu, valid);
+        if (valid) add_aggregated(counts, indices[i], active);
+    }
+}
+
+// Radix select of the K-th largest count, 16 bits at a time.  hi == ~0u: every referenced
+// column, binned by the upper 16 bits of its count; otherwise the columns whose count has `hi`
+// in its upper bits, binned by the lower 16.
+__global__ void hot_count_hist_kernel(const uint32_t* __restrict__ counts, uint32_t cols,
+                                      uint32_t hi, uint32_t* __restrict__ hist) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t base = blockIdx.x * (uint64_t)blockDim.x + (threadIdx.x & ~31u); base < cols;
+         base += stride) {
+        const uint64_t i = base + (threadIdx.x & 31);
+        const uint32_t c = i < cols ? counts[i] : 0u;
+        const bool take = c > 0 && (hi == ~0u || (c >> 16) == hi);
+        const unsigned active = __ballot_sync(0xffffffffu, take);
+        if (take) add_aggregated(hist, hi == ~0u ? c >> 16 : c & 0xffffu, active);
+    }
+}
+
+// The K hot columns: every count above `thr`, then the first `ties` columns (in column order)
+// whose count equals it.  tie_rank == nullptr: flag the ties themselves (their scan is the rank)
+__global__ void hot_flag_kernel(const uint32_t* __restrict__ counts, uint32_t cols, uint32_t thr,
+                                const uint32_t* __restrict__ tie_rank, uint32_t ties,
+                                uint8_t* __restrict__ flag) {
+    const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i >= cols) return;
+    const uint32_t c = counts[i];
+    flag[i] = tie_rank ? (c > thr || (c == thr && tie_rank[i] < ties)) : c == thr;
+}
+
+// counts -> the tag map (a column's entry in the SpMV's index stream), hot_col[slot] = column,
+// hot_nnz = the references the hot set serves
+__global__ void hot_map_kernel(uint32_t* __restrict__ counts_map, uint32_t cols,
+                               const uint8_t* __restrict__ sel, const uint32_t* __restrict__ slot,
+                               uint32_t* __restrict__ hot_col, unsigned long long* hot_nnz) {
+    const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i >= cols) return;
+    if (sel[i]) {
+        const uint32_t q = slot[i];
+        atomicAdd(hot_nnz, (unsigned long long)counts_map[i]);
+        hot_col[q] = (uint32_t)i;
+        counts_map[i] = HOT_TAG | q;
+    } else {
+        counts_map[i] = (uint32_t)i;
+    }
+}
+
+__global__ void hot_tag_kernel(const uint32_t* __restrict__ indices, uint64_t nnz,
+                               const uint32_t* __restrict__ map, uint32_t* __restrict__ tagged) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < nnz; i += stride)
+        tagged[i] = map[indices[i]];
+}
+
+// Builds m's hot set, or leaves the mirror without one (n_hot = 0) where `auto` says it does not
+// pay or a buffer cannot be allocated -- the SpMV then runs exactly as without it.
+int spmv_prepare_hot(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s) {
+    const SpmvHot cfg = spmv_hot();
+    if (cfg.k == 0 || m->nnz == 0 || m->cols == 0 || m->cols >= HOT_TAG) return SPRS_B200_OK;
+    if (!cfg.forced && m->nnz < SPMV_HOT_MIN_NNZ) return SPRS_B200_OK;
+    const uint32_t cols = (uint32_t)m->cols;
+    uint32_t *counts = nullptr, *hist = nullptr, *slot = nullptr, *hot_col = nullptr,
+             *hot_idx = nullptr;
+    uint8_t* flag = nullptr;
+    unsigned long long* d_hot_nnz = nullptr;
+    const unsigned grid_nnz =
+        (unsigned)std::min<uint64_t>((m->nnz + 255) / 256, (uint64_t)ctx->sm_count * 16);
+    const unsigned grid_cols = (unsigned)((cols + 255) / 256);
+    // returns with m->n_hot still 0 wherever the mirror gets no hot set
+    auto build = [&]() -> int {
+        if (cudaMalloc((void**)&counts, cols * sizeof(uint32_t)) != cudaSuccess ||
+            cudaMalloc((void**)&hist, 65536 * sizeof(uint32_t)) != cudaSuccess ||
+            cudaMalloc((void**)&flag, cols) != cudaSuccess ||
+            cudaMalloc((void**)&slot, (cols + 1ull) * sizeof(uint32_t)) != cudaSuccess ||
+            cudaMalloc((void**)&d_hot_nnz, sizeof(unsigned long long)) != cudaSuccess)
+            return SPRS_B200_OK;  // not enough memory for the build: no hot set
+        // ---- references per column, then the count of the K-th most referenced column
+        SPRS_CUDA(ctx, cudaMemsetAsync(counts, 0, cols * sizeof(uint32_t), s));
+        SPRS_CUDA(ctx, cudaMemsetAsync(hist, 0, 65536 * sizeof(uint32_t), s));
+        SPRS_CUDA(ctx, cudaMemsetAsync(d_hot_nnz, 0, sizeof(unsigned long long), s));
+        hot_count_kernel<<<grid_nnz, 256, 0, s>>>(m->d_indices, m->nnz, counts);
+        hot_count_hist_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, ~0u, hist);
+        ctx->launches += 2;
+        std::vector<uint32_t> h(65536);
+        SPRS_CUDA(ctx, cudaMemcpyAsync(h.data(), hist, 65536 * sizeof(uint32_t),
+                                       cudaMemcpyDeviceToHost, s));
+        SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+        uint64_t above = 0, referenced = 0;
+        for (uint32_t b = 0; b < 65536; ++b) referenced += h[b];
+        uint32_t k = cfg.k, thr = 1, ties = 0xffffffffu;  // K or fewer referenced columns: all
+        if (referenced > k) {
+            uint32_t bhi = 65535;  // (the loops stop: the bins hold more than K columns)
+            while (above + h[bhi] < k) above += h[bhi--];
+            SPRS_CUDA(ctx, cudaMemsetAsync(hist, 0, 65536 * sizeof(uint32_t), s));
+            hot_count_hist_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, bhi, hist);
+            ctx->launches += 1;
+            SPRS_CUDA(ctx, cudaMemcpyAsync(h.data(), hist, 65536 * sizeof(uint32_t),
+                                           cudaMemcpyDeviceToHost, s));
+            SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+            uint32_t blo = 65535;
+            while (above + h[blo] < k) above += h[blo--];
+            thr = (bhi << 16) | blo;
+            ties = k - (uint32_t)above;  // columns of count thr to take, in column order
+        } else {
+            k = (uint32_t)referenced;
+        }
+        // ---- select, slots in column order, tag map
+        hot_flag_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, thr, nullptr, 0, flag);
+        ctx->launches += 1;
+        SPRS_TRY((device_exclusive_scan<uint8_t, uint32_t>(ctx, flag, cols, slot, s)));
+        hot_flag_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, thr, slot, ties, flag);
+        ctx->launches += 1;
+        SPRS_TRY((device_exclusive_scan<uint8_t, uint32_t>(ctx, flag, cols, slot, s)));
+        if (cudaMalloc((void**)&hot_col, k * sizeof(uint32_t)) != cudaSuccess) return SPRS_B200_OK;
+        hot_map_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, flag, slot, hot_col, d_hot_nnz);
+        ctx->launches += 1;
+        unsigned long long hot_nnz = 0;
+        SPRS_CUDA(ctx, cudaMemcpyAsync(&hot_nnz, d_hot_nnz, sizeof(hot_nnz), cudaMemcpyDeviceToHost, s));
+        SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+        if (!cfg.forced && (double)hot_nnz < SPMV_HOT_MIN_SHARE * (double)m->nnz) return SPRS_B200_OK;
+        // ---- the tagged index stream (+4 bytes per non-zero)
+        if (cudaMalloc((void**)&hot_idx, m->nnz * sizeof(uint32_t) + 16) != cudaSuccess)
+            return SPRS_B200_OK;
+        hot_tag_kernel<<<grid_nnz, 256, 0, s>>>(m->d_indices, m->nnz, counts, hot_idx);
+        ctx->launches += 1;
+        SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+        SPRS_CUDA(ctx, cudaGetLastError());
+        m->d_hot_col = hot_col;
+        m->d_hot_idx = hot_idx;
+        m->n_hot = k;
+        return SPRS_B200_OK;
+    };
+    const int st = build();
+    if (m->n_hot == 0) {
+        cudaGetLastError();  // (a failed allocation leaves an error behind: it is not one here)
+        if (hot_col) cudaFree(hot_col);
+        if (hot_idx) cudaFree(hot_idx);
+    }
+    if (counts) cudaFree(counts);
+    if (hist) cudaFree(hist);
+    if (flag) cudaFree(flag);
+    if (slot) cudaFree(slot);
+    if (d_hot_nnz) cudaFree(d_hot_nnz);
+    return st;
 }
 
 int check_spmv_args(sprs_b200_ctx* ctx, const sprs_b200_csmat* m) {
@@ -528,7 +780,7 @@ int check_spmv_args(sprs_b200_ctx* ctx, const sprs_b200_csmat* m) {
 
 int spmv_tile_nnz() { return spmv_variant().wt; }
 
-int spmv_prepare(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s) {
+int spmv_prepare(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, bool hot_set) {
     if (m->storage != SPRS_B200_CSR) return SPRS_B200_OK;  // CSC mirrors are converted first
     const uint32_t w = (uint32_t)spmv_tile_nnz();  // cost units per tile
     const uint32_t row_cost = (uint32_t)spmv_variant().row_cost;
@@ -549,6 +801,7 @@ int spmv_prepare(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s) {
                                                        (uint64_t*)m->d_tile_k);
     ctx->launches += 1;
     SPRS_CUDA(ctx, cudaGetLastError());
+    if (hot_set) SPRS_TRY(spmv_prepare_hot(ctx, m, s));
     return SPRS_B200_OK;
 }
 

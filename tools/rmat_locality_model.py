@@ -18,9 +18,10 @@ A, B, C_, D = 0.57, 0.19, 0.19, 0.05
 def sample_rows(rng, n_blocks, block_rows):
     out = []
     for _ in range(n_blocks):
-        bits = rng.random(SCALE) < (C_ + D)
-        r0 = int(sum(int(b) << (SCALE - 1 - i) for i, b in enumerate(bits)))
-        r0 = (r0 // block_rows) * block_rows
+        # blocks are drawn UNIFORMLY over the rows: each row's weight is its own non-zero count
+        # below (drawing blocks with R-MAT's row bias as well would count that bias twice and
+        # understate the share of the hot columns)
+        r0 = int(rng.integers(0, N // block_rows)) * block_rows
         for r in range(r0, min(r0 + block_rows, N)):
             rb = np.array([(r >> (SCALE - 1 - i)) & 1 for i in range(SCALE)], dtype=bool)
             k = int(rb.sum())
