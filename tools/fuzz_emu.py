@@ -1,11 +1,18 @@
 """Structure fuzzer for the kernels' LOGIC on the CPU emulator (tests/emu; test infrastructure).
 
 Random small matrices whose row lengths are drawn to sit ON the kernels' internal boundaries --
-the SpMV tile size (256 non-zeros and the other variants), the 24/25-row register path, lane
-groups, the warp/CTA/bitmap bins of the SpGEMM -- are pushed through the C ABI of the emulated
-library and compared with the oracle: SpMV (values within the parity gate, bit-exact where
-the design promises it), SpMM (bit-exact), SpGEMM (indptr / indices bit-exact, values within
-the gate), CSR<->CSC (bit-exact), triplets (pattern bit-exact), CSR x sparse vector (bit-exact).
+the SpMV merge-path tile (1024 cost units, a row end costing 16: a tile is ~1000 non-zeros or 64
+row ends), its tiny rows (<= 8 non-zeros, one lane each), the lane groups G = 4 / 8 / 16 / 32 and
+their switch to the whole warp above 16 G non-zeros, the 31-row blocks; the SpMM column panels
+(64 / 128 columns per pass); the SpGEMM bins (128 / 1024 C entries, 4096 A non-zeros, 16384-column
+panels) -- are pushed through the C ABI of the emulated library and compared with the oracle:
+SpMV (values within the parity gate, bit-exact where the design promises it), SpMM (bit-exact),
+SpGEMM (indptr / indices bit-exact, values within the gate), CSR<->CSC (bit-exact), triplets
+(pattern bit-exact), CSR x sparse vector (bit-exact).
+
+Every odd seed runs in INTEGER mode (tests/exact.py): A, B, x and y0 are small integers, every
+sum is exact in f64 whatever its order, and the SpMV, SpGEMM and dense-product checks become
+bit-equality.
 
     python tools/fuzz_emu.py --seconds 300 [--seed 1] [--schedule random:3]
 
@@ -21,6 +28,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+import exact  # noqa: E402  (tests/exact.py: integer-valued inputs)
 
 
 def setup(schedule):
@@ -39,10 +47,9 @@ def setup(schedule):
     return sprs_b200, O
 
 
-BOUNDARY_LENS = [0, 0, 0, 1, 1, 2, 3, 5, 6, 7, 8, 9, 10, 11, 12, 13, 16, 24, 31, 32, 33, 47, 48, 49,
-                 63, 64, 65, 95, 96, 97, 127, 128, 129, 191, 192, 193, 255, 256, 257, 319, 320,
-                 321, 383, 384, 385, 511, 512, 513, 767, 768, 769, 1023, 1024, 1025, 1151, 1152, 1153, 2047,
-                 2048, 2049]
+BOUNDARY_LENS = [0, 0, 0, 1, 1, 2, 3, 5, 7, 8, 9, 10, 15, 16, 17, 31, 32, 33, 63, 64, 65, 127, 128,
+                 129, 255, 256, 257, 511, 512, 513, 1007, 1008, 1009, 1023, 1024, 1025, 1129, 1130,
+                 2047, 2048, 2049, 4095, 4096, 4097]
 
 
 def row_lengths(rng, rows, cols):
@@ -52,20 +59,20 @@ def row_lengths(rng, rows, cols):
         lens = rng.choice(BOUNDARY_LENS, rows)
     elif mode == 1:   # constant short rows (register path / group sizes)
         lens = np.full(rows, rng.choice([1, 2, 3, 4, 6, 8, 12, 16, 24, 32, 42, 43, 48, 64, 96, 128]))
-    elif mode == 2:   # long empty stretches around tile boundaries
-        lens = rng.choice([0, 0, 0, 0, 384, 383, 256, 255, 1, 2, 768, 32, 64], rows)
+    elif mode == 2:   # long empty stretches around tile boundaries (64 row ends fill a tile)
+        lens = rng.choice([0, 0, 0, 0, 1008, 1007, 1009, 496, 1, 2, 2032, 32, 64], rows)
     elif mode == 3:   # poisson
         lens = rng.poisson(rng.choice([1, 4, 20, 60]), rows)
     elif mode == 4:   # hubs + dust
         lens = rng.choice([0, 1, 2, 3], rows)
         for _ in range(rng.integers(1, 4)):
             lens[rng.integers(0, rows)] = rng.choice([384, 385, 700, 1152, 1500, 3000, 4100])
-    else:             # tile-aligned prefix sums: every row ends exactly on a multiple of 128/384
-        lens = rng.choice([128, 256, 384, 768, 0, 32, 64, 0], rows)
+    else:             # rows of cost 512 / 1024 (length + 16): many rows end exactly on a cut
+        lens = rng.choice([496, 1008, 2032, 0, 48, 112, 0], rows)
     return np.minimum(lens.astype(np.int64), cols)
 
 
-def make_csr(rng, rows, cols, lens):
+def make_csr(rng, rows, cols, lens, integer=False):
     indptr = np.zeros(rows + 1, dtype=np.int64)
     np.cumsum(lens, out=indptr[1:])
     indices = np.empty(indptr[-1], dtype=np.int64)
@@ -73,6 +80,8 @@ def make_csr(rng, rows, cols, lens):
         n = lens[r]
         if n:
             indices[indptr[r]:indptr[r + 1]] = np.sort(rng.choice(cols, size=n, replace=False))
+    if integer:
+        return indptr.astype(np.uint32), indices.astype(np.uint32), exact.int_csr_data(indptr, rng.integers(1 << 30))
     data = rng.standard_normal(indptr[-1])
     # a few special values: exact zeros, huge / tiny magnitudes
     if data.size:
@@ -81,7 +90,16 @@ def make_csr(rng, rows, cols, lens):
     return indptr.astype(np.uint32), indices.astype(np.uint32), data
 
 
-def gate(got, ref, bound, what):
+def gate(got, ref, bound, what, bits=False):
+    """the parity gate; bits=True (integer mode: every sum exact) -> bit-equality instead"""
+    if bits:
+        g, r = np.ascontiguousarray(got, dtype=np.float64), np.ascontiguousarray(ref, dtype=np.float64)
+        bad = g.view(np.uint64) != r.view(np.uint64)
+        if bad.any():
+            i = int(np.flatnonzero(bad.ravel())[0])
+            return "%s: element %d got %r want %r (integer data: must be bit-exact)" % (
+                what, i, g.flat[i], r.flat[i])
+        return None
     bad = ~(np.abs(got - ref) <= 1e-6 * bound + 1e-300)
     bad &= ~(np.isnan(got) & np.isnan(ref))
     bad &= ~((got == ref))     # equal infinities
@@ -161,21 +179,22 @@ def one_case(sp, O, seed):
     if rng.integers(0, 4) == 0:
         cols = rows  # square: also feeds the solver
     lens = row_lengths(rng, rows, cols)
-    ip, ind, d = make_csr(rng, rows, cols, lens)
+    integer = seed % 2 == 1  # small integers: every sum exact, the products' checks bit-equality
+    ip, ind, d = make_csr(rng, rows, cols, lens, integer)
     idx = rng.choice([np.uint32, np.uint64])
     a = sp.CsMat.new((rows, cols), ip.astype(idx), ind.astype(idx), d)
     errs = []
     # ---- SpMV (accumulating free function and the operator)
     finite = np.where(np.abs(d) > 1e200, 1.0, d)  # keep the gate meaningful: no overflow sums
     af = sp.CsMat.new((rows, cols), ip, ind, finite)
-    x = rng.standard_normal(cols)
-    y0 = rng.standard_normal(rows)
+    x = exact.x_values(np.arange(cols, dtype=np.int64), seed) if integer else rng.standard_normal(cols)
+    y0 = exact.y0_values(rows, seed) if integer else rng.standard_normal(rows)
     got = y0.copy()
     sp.prod.mul_acc_mat_vec_csr(af, x, got)
     ref, bound = y0.copy(), np.abs(y0)
     O.mul_acc_mat_vec_csr(ip, ind, finite, x, ref)
     O.mul_acc_mat_vec_csr(ip, ind, np.abs(finite), np.abs(x), bound)
-    e = gate(got, ref, bound, "spmv")
+    e = gate(got, ref, bound, "spmv", integer)
     if e:
         errs.append(e)
     elif lens.max() <= 6 and int(ip[-1]) + 16 * rows < 1024:
@@ -193,7 +212,8 @@ def one_case(sp, O, seed):
             errs.append(e)
     # ---- SpMM: bit-exact, k on both sides of the k >= 8 rule
     k = int(rng.choice([1, 3, 8, 9, 32, 33, 64, 70]))
-    b = rng.standard_normal((cols, k))
+    b = exact.mat_values(np.arange(cols * k, dtype=np.int64), seed).reshape(cols, k) if integer \
+        else rng.standard_normal((cols, k))
     c = af * b
     cref = np.zeros((rows, k))
     O.csr_mulacc_dense_rowmaj(ip, ind, finite, b, cref)
@@ -203,7 +223,7 @@ def one_case(sp, O, seed):
     else:
         cb = np.zeros((rows, k))
         O.csr_mulacc_dense_rowmaj(ip, ind, np.abs(finite), np.abs(b), cb)
-        e = gate(np.asarray(c), cref, cb, "spmm-colmaj k=%d" % k)
+        e = gate(np.asarray(c), cref, cb, "spmm-colmaj k=%d" % k, integer)
         if e:
             errs.append(e)
     # ---- CSC operands (device CSC -> CSR, then the CSR kernels: same ascending-column sums)
@@ -214,11 +234,13 @@ def one_case(sp, O, seed):
     refc, bc = np.zeros(rows), np.zeros(rows)
     O.mul_acc_mat_vec_csr(ip, ind, finite, x, refc)
     O.mul_acc_mat_vec_csr(ip, ind, np.abs(finite), np.abs(x), bc)
-    e = gate(yc, refc, bc, "csc spmv")
+    e = gate(yc, refc, bc, "csc spmv", integer)
     if e:
         errs.append(e)
     kk = int(rng.choice([8, 13, 40]))
     big = rng.standard_normal((2 * cols + 1, 2 * kk + 3))
+    if integer:
+        big = exact.mat_values(np.arange(big.size, dtype=np.int64), seed + 1).reshape(big.shape)
     view = big[::2][:cols, ::-2][:, :kk] if rng.integers(0, 2) else np.asfortranarray(big[:cols, :kk])
     outbig = np.zeros((rows * 2 + 1, kk + 2))
     out = outbig[1::2][:rows, 1:kk + 1]
@@ -228,7 +250,7 @@ def one_case(sp, O, seed):
     O.csr_mulacc_dense_rowmaj(ip, ind, finite, np.ascontiguousarray(view), want)
     wb = np.zeros((rows, kk))
     O.csr_mulacc_dense_rowmaj(ip, ind, np.abs(finite), np.abs(np.ascontiguousarray(view)), wb)
-    e = gate(np.ascontiguousarray(out), want, wb, "csc dense product on strided views")
+    e = gate(np.ascontiguousarray(out), want, wb, "csc dense product on strided views", integer)
     if e:
         errs.append(e)
     if outbig[0::2].any() or outbig[:, 0].any() or outbig[:, kk + 1].any():
@@ -258,7 +280,7 @@ def one_case(sp, O, seed):
     # 9000 / 23000 columns: C rows beyond 4096 entries -> dense shared-memory panels (1 and 2)
     bcols = int(rng.choice([1, 9, 300, 2500, 2500, 9000, 23000]))
     blens = row_lengths(rng, cols, bcols)
-    bip, bind, bd = make_csr(rng, cols, bcols, blens)
+    bip, bind, bd = make_csr(rng, cols, bcols, blens, integer)
     bd = np.where(np.abs(bd) > 1e200, 1.0, bd)
     bm = sp.CsMat.new((cols, bcols), bip.astype(idx), bind.astype(idx), bd)
     af2 = sp.CsMat.new((rows, cols), ip.astype(idx), ind.astype(idx), finite)
@@ -270,7 +292,7 @@ def one_case(sp, O, seed):
     else:
         _, _, cb = O.mul_csr_csr((rows, cols), (ip, ind, np.abs(finite)), (cols, bcols),
                                  (bip, bind, np.abs(bd)), threads=1)
-        e = gate(cm.data, cd, cb, "spgemm values")
+        e = gate(cm.data, cd, cb, "spgemm values", integer)
         if e:
             errs.append(e)
         # storage dispatch (csmat.rs:1895-1949): CSC operands route through transposes; the
@@ -285,7 +307,7 @@ def one_case(sp, O, seed):
                 g = got.to_other_storage() if want_csc else got
                 if not (np.array_equal(g.indptr, cip) and np.array_equal(g.indices, cind)):
                     errs.append("spgemm dispatch: pattern differs from CSR x CSR")
-                elif gate(g.data, cd, cb, "spgemm dispatch values"):
+                elif gate(g.data, cd, cb, "spgemm dispatch values", integer):
                     errs.append("spgemm dispatch: values differ from CSR x CSR")
     # ---- row slices: slice_outer + proper_indptr upload (slicing.rs:65-89), SpMV on the view
     if rows >= 3:
@@ -293,7 +315,7 @@ def one_case(sp, O, seed):
         hi = int(rng.integers(lo + 1, rows + 1))
         sl = af.slice_outer(lo, hi)
         ys = sl * x
-        e = gate(ys, refc[lo:hi], bc[lo:hi], "spmv on a row slice")
+        e = gate(ys, refc[lo:hi], bc[lo:hi], "spmv on a row slice", integer)
         if e:
             errs.append(e)
     # ---- BiCGSTAB on a diagonally dominant system built from the same pattern
