@@ -329,7 +329,9 @@ int sprs_b200_spgemm_free(sprs_b200_spgemm* plan);
  * The matrix may be CSR or CSC (both sum A*v in ascending column order) and must be
  * square with n rows (else DIMENSION, the reference's "Dimension mismatch" panic).  The
  * solver BORROWS the matrix mirror: keep it alive until bicgstab_free.  x0 and b are
- * copied (host pointers for _new, device pointers for _new_dev).                      */
+ * copied (host pointers for _new, device pointers for _new_dev).  _new_dev copies them on
+ * the ctx's own stream and takes no stream argument, so the device arrays must be COMPLETE
+ * when the call is made: synchronise the stream that produced them first.              */
 typedef struct sprs_b200_bicgstab sprs_b200_bicgstab;
 enum {
     SPRS_B200_BICGSTAB_X = 0,    /* x()    latest solution            (bicgstab.rs:272) */

@@ -27,6 +27,7 @@ def main():
     lib = ctx.lib
     x0 = G.normal_vector(ctx, n, 1)
     b = G.normal_vector(ctx, n, 2)
+    G._sync()  # new_dev copies x0 / b on the library's stream: torch's must have written them
     h = C.c_void_p()
     ctx.check(lib.sprs_b200_bicgstab_new_dev(ctx.h, a.mirror.h, C.c_void_p(x0.data_ptr()),
                                              C.c_void_p(b.data_ptr()), n, C.byref(h)))
