@@ -116,6 +116,20 @@ int sprs_b200_csmat_check_structure(sprs_b200_ctx* ctx, const sprs_b200_csmat* m
 int sprs_b200_csmat_to_other_storage(sprs_b200_ctx* ctx, const sprs_b200_csmat* m,
                                      sprs_b200_csmat** out);
 
+/* ---- sparse (+, -, Hadamard) sparse and sparse * scalar, device-resident result --------
+ * The host-buffer form needs no symbol of its own: read csmat_nnz of the result, allocate,
+ * and csmat_download it.                                                                    */
+enum { SPRS_B200_BINOP_ADD = 0, SPRS_B200_BINOP_SUB = 1, SPRS_B200_BINOP_MUL = 2 };
+/* csmat_binop (binop.rs:178-271): new mirror C, storage of lhs; entries whose result is 0.0 dropped.
+ * Same storage required (else STORAGE; the host mirrors convert rhs for Add/Sub), same shape
+ * (else DIMENSION, checked first), op outside the enum -> ARGUMENT.  Blocking, ctx stream;
+ * operands adopted with from_device must be complete when called.                          */
+int sprs_b200_csmat_binop(sprs_b200_ctx* ctx, const sprs_b200_csmat* lhs,
+                          const sprs_b200_csmat* rhs, int op, sprs_b200_csmat** out);
+/* &A * s (binop.rs:132-163 -> CsMatBase::map): same structure, data[k]*s, zeros kept */
+int sprs_b200_csmat_scale(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, double s,
+                          sprs_b200_csmat** out);
+
 /* ---- sparse x dense vector, HOST buffers (copies are part of the call) --------
  * prod::mul_acc_mat_vec_csr(mat, in_vec, res_vec)  prod.rs:103-127 : y += A x
  * prod::mul_acc_mat_vec_csc                        prod.rs:74-99

@@ -9,6 +9,7 @@
 //   &a * &b  (sparse, Array2, Array1, CsVec), dot()    csmat.rs:1866-2178, vec.rs:1084-1131
 //   sprs::prod::mul_acc_mat_vec_csr / csr_mulacc_dense_{row,col}maj / ...   prod.rs
 //   sprs::smmp::mul_csr_csr                            smmp.rs:196-237
+//   &a + &b, &a - &b, &a * s, binop::mul_mat_same_storage   binop.rs:20-163
 //
 // Contract violations throw sprs::Panic carrying the reference's panic message
 // ("Dimension mismatch", "Storage mismatch"; Guidelines.rst:9-27); device failures
@@ -369,6 +370,68 @@ CsMatI<I, Iptr> operator*(const CsMatI<I, Iptr>& lhs, const CsMatI<I, Iptr>& rhs
         return smmp::mul_csr_csr(rhs_csc.transpose_view(), lhs.transpose_view()).transpose_into();
     }
     return smmp::mul_csr_csr(rhs.transpose_view(), lhs.transpose_view()).transpose_into();
+}
+
+// ---- the `impl Add / Sub / Mul<N>` blocks and binop::mul_mat_same_storage (binop.rs:20-163)
+namespace binop {
+namespace detail {
+// csmat_binop (binop.rs:178-271) on the device: the result in lhs's storage, entries whose
+// result is 0.0 dropped; `rhs_dev` has lhs's storage
+template <class I, class Iptr>
+CsMatI<I, Iptr> csmat_binop(const CsMatI<I, Iptr>& lhs, const sprs_b200_csmat* rhs_dev, int op) {
+    Context& ctx = Context::thread_default();
+    sprs_b200_csmat* c = nullptr;
+    ctx.check(sprs_b200_csmat_binop(ctx.handle(), lhs.device(), rhs_dev, op, &c));
+    CsMatI<I, Iptr> out = CsMatI<I, Iptr>::download(ctx, c, lhs.storage(), lhs.rows(), lhs.cols());
+    sprs_b200_csmat_free(c);
+    return out;
+}
+// Add / Sub: the shapes are asserted first, then rhs is converted to lhs's storage
+template <class I, class Iptr>
+CsMatI<I, Iptr> add_or_sub(const CsMatI<I, Iptr>& lhs, const CsMatI<I, Iptr>& rhs, int op) {
+    if (lhs.rows() != rhs.rows() || lhs.cols() != rhs.cols()) throw Panic("Dimension mismatch");
+    if (lhs.storage() == rhs.storage()) return csmat_binop(lhs, rhs.device(), op);
+    Context& ctx = Context::thread_default();
+    sprs_b200_csmat* t = nullptr;
+    ctx.check(sprs_b200_csmat_to_other_storage(ctx.handle(), rhs.device(), &t));
+    sprs_b200_csmat* c = nullptr;
+    const int st = sprs_b200_csmat_binop(ctx.handle(), lhs.device(), t, op, &c);
+    sprs_b200_csmat_free(t);
+    ctx.check(st);
+    CsMatI<I, Iptr> out = CsMatI<I, Iptr>::download(ctx, c, lhs.storage(), lhs.rows(), lhs.cols());
+    sprs_b200_csmat_free(c);
+    return out;
+}
+}  // namespace detail
+
+// binop::mul_mat_same_storage (binop.rs:115-130): element-wise product; mixed storage panics
+template <class I, class Iptr>
+CsMatI<I, Iptr> mul_mat_same_storage(const CsMatI<I, Iptr>& lhs, const CsMatI<I, Iptr>& rhs) {
+    if (lhs.rows() != rhs.rows() || lhs.cols() != rhs.cols()) throw Panic("Dimension mismatch");
+    if (lhs.storage() != rhs.storage()) throw Panic("Storage mismatch");
+    return detail::csmat_binop(lhs, rhs.device(), SPRS_B200_BINOP_MUL);
+}
+}  // namespace binop
+
+// `&A + &B` (binop.rs:20-65)
+template <class I, class Iptr>
+CsMatI<I, Iptr> operator+(const CsMatI<I, Iptr>& lhs, const CsMatI<I, Iptr>& rhs) {
+    return binop::detail::add_or_sub(lhs, rhs, SPRS_B200_BINOP_ADD);
+}
+// `&A - &B` (binop.rs:67-112)
+template <class I, class Iptr>
+CsMatI<I, Iptr> operator-(const CsMatI<I, Iptr>& lhs, const CsMatI<I, Iptr>& rhs) {
+    return binop::detail::add_or_sub(lhs, rhs, SPRS_B200_BINOP_SUB);
+}
+// `&A * s` (binop.rs:132-163 -> CsMatBase::map): same structure, every value times s
+template <class I, class Iptr>
+CsMatI<I, Iptr> operator*(const CsMatI<I, Iptr>& a, double s) {
+    Context& ctx = Context::thread_default();
+    sprs_b200_csmat* c = nullptr;
+    ctx.check(sprs_b200_csmat_scale(ctx.handle(), a.device(), s, &c));
+    CsMatI<I, Iptr> out = CsMatI<I, Iptr>::download(ctx, c, a.storage(), a.rows(), a.cols());
+    sprs_b200_csmat_free(c);
+    return out;
 }
 // `&A * &x`, x: Array1 (csmat.rs:2119-2160)
 template <class I, class Iptr>

@@ -14,6 +14,9 @@ use std::os::raw::{c_char, c_double, c_int, c_void};
 
 pub const SPRS_B200_CSR: c_int = 0;
 pub const SPRS_B200_CSC: c_int = 1;
+pub const SPRS_B200_BINOP_ADD: c_int = 0;
+pub const SPRS_B200_BINOP_SUB: c_int = 1;
+pub const SPRS_B200_BINOP_MUL: c_int = 2;
 pub const SPRS_B200_OK: c_int = 0;
 pub const SPRS_B200_ERR_DIMENSION: c_int = 1;
 pub const SPRS_B200_ERR_STORAGE: c_int = 2;
@@ -50,6 +53,12 @@ extern "C" {
         indptr_bytes: c_int, indices: *mut c_void, index_bytes: c_int, data: *mut c_double) -> c_int;
     pub fn sprs_b200_csmat_to_other_storage(
         ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat, out: *mut *mut sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_csmat_binop(
+        ctx: *mut sprs_b200_ctx, lhs: *const sprs_b200_csmat, rhs: *const sprs_b200_csmat,
+        op: c_int, out: *mut *mut sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_csmat_scale(
+        ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat, s: c_double,
+        out: *mut *mut sprs_b200_csmat) -> c_int;
     pub fn sprs_b200_mul_acc_mat_vec_csr(
         ctx: *mut sprs_b200_ctx, mat: *const sprs_b200_csmat, in_vec: *const c_double, in_len: u64,
         res_vec: *mut c_double, res_len: u64) -> c_int;

@@ -8,6 +8,8 @@
 //! let y: Array1<f64> = &a * &x;             // csmat.rs:2119-2160 -> sprs_b200_mul_mat_vec
 //! let c: Array2<f64> = &a * &b;             // csmat.rs:1989-2048 (k >= 8 -> rowmaj, C order)
 //! let p: CsMatI<f64, I, Iptr> = &a * &b_sp; // csmat.rs:1866-1949 -> smmp::mul_csr_csr
+//! let s: CsMatI<f64, I, Iptr> = &a + &b_sp; // binop.rs:20-112 (also `-`, `&a * 2.0`,
+//!                                           // binop::mul_mat_same_storage)
 //! ```
 //! Contract violations panic with the reference's messages (Guidelines.rst:9-27);
 //! device failures are `LinalgError::ThirdPartyError(code, msg)` (errors.rs:70).
@@ -172,6 +174,75 @@ pub fn mul_csr_csr<I: SpIndex, Iptr: SpIndex>(lhs: &DeviceCsMat<I, Iptr>, rhs: &
 impl<'a, 'b, I: SpIndex, Iptr: SpIndex> Mul<&'b DeviceCsMat<I, Iptr>> for &'a DeviceCsMat<I, Iptr> {
     type Output = CsMatI<f64, I, Iptr>;
     fn mul(self, rhs: &'b DeviceCsMat<I, Iptr>) -> Self::Output { mul_csr_csr(self, rhs) }
+}
+
+// ---- binop.rs:20-163: `&A + &B`, `&A - &B`, `&A * s` and binop::mul_mat_same_storage.  The
+// device result (lhs storage, entries whose result is 0.0 dropped; map keeps every entry) is
+// downloaded into Vecs the caller side allocates, like mul_csr_csr.
+fn download_result<I: SpIndex, Iptr: SpIndex>(c: *mut ffi::sprs_b200_ctx, m: *mut ffi::sprs_b200_csmat,
+                                              like: &CsMatI<f64, I, Iptr>) -> CsMatI<f64, I, Iptr> {
+    let nnz = unsafe { ffi::sprs_b200_csmat_nnz(m) } as usize;
+    let mut indptr = vec![Iptr::zero(); like.outer_dims() + 1];
+    let mut indices = vec![I::zero(); nnz];
+    let mut data = vec![0f64; nnz];
+    let st = unsafe {
+        ffi::sprs_b200_csmat_download(c, m, indptr.as_mut_ptr() as *mut c_void,
+            std::mem::size_of::<Iptr>() as i32, indices.as_mut_ptr() as *mut c_void,
+            std::mem::size_of::<I>() as i32, data.as_mut_ptr())
+    };
+    unsafe { ffi::sprs_b200_csmat_free(m); }
+    check(c, st).expect("sprs_b200 device error");
+    // sorted unique in-range indices by construction (binop.rs:210-217 new_trusted)
+    CsMatI::new_trusted(like.storage(), (like.rows(), like.cols()), indptr, indices, data)
+}
+
+fn csmat_binop<I: SpIndex, Iptr: SpIndex>(lhs: &DeviceCsMat<I, Iptr>, rhs: &DeviceCsMat<I, Iptr>, op: i32) -> CsMatI<f64, I, Iptr> {
+    // binop.rs:195-199: shapes first, then storage; Add / Sub convert rhs (binop.rs:20-112)
+    assert!(lhs.host.rows() == rhs.host.rows() && lhs.host.cols() == rhs.host.cols(), "Dimension mismatch");
+    CTX.with(|c| {
+        let mut conv = std::ptr::null_mut();
+        let rdev = if lhs.host.storage() == rhs.host.storage() { rhs.dev } else {
+            assert!(op != ffi::SPRS_B200_BINOP_MUL, "Storage mismatch");
+            check(c.0, unsafe { ffi::sprs_b200_csmat_to_other_storage(c.0, rhs.dev, &mut conv) })
+                .expect("sprs_b200 device error");
+            conv
+        };
+        let mut out = std::ptr::null_mut();
+        let st = unsafe { ffi::sprs_b200_csmat_binop(c.0, lhs.dev, rdev, op, &mut out) };
+        if !conv.is_null() { unsafe { ffi::sprs_b200_csmat_free(conv); } }
+        check(c.0, st).expect("sprs_b200 device error");
+        download_result(c.0, out, &lhs.host)
+    })
+}
+
+impl<'a, 'b, I: SpIndex, Iptr: SpIndex> std::ops::Add<&'b DeviceCsMat<I, Iptr>> for &'a DeviceCsMat<I, Iptr> {
+    type Output = CsMatI<f64, I, Iptr>;
+    fn add(self, rhs: &'b DeviceCsMat<I, Iptr>) -> Self::Output { csmat_binop(self, rhs, ffi::SPRS_B200_BINOP_ADD) }
+}
+impl<'a, 'b, I: SpIndex, Iptr: SpIndex> std::ops::Sub<&'b DeviceCsMat<I, Iptr>> for &'a DeviceCsMat<I, Iptr> {
+    type Output = CsMatI<f64, I, Iptr>;
+    fn sub(self, rhs: &'b DeviceCsMat<I, Iptr>) -> Self::Output { csmat_binop(self, rhs, ffi::SPRS_B200_BINOP_SUB) }
+}
+// `&A * s` (binop.rs:132-163 -> CsMatBase::map): same structure, every value times s
+impl<'a, I: SpIndex, Iptr: SpIndex> Mul<f64> for &'a DeviceCsMat<I, Iptr> {
+    type Output = CsMatI<f64, I, Iptr>;
+    fn mul(self, s: f64) -> Self::Output {
+        CTX.with(|c| {
+            let mut out = std::ptr::null_mut();
+            check(c.0, unsafe { ffi::sprs_b200_csmat_scale(c.0, self.dev, s, &mut out) })
+                .expect("sprs_b200 device error");
+            download_result(c.0, out, &self.host)
+        })
+    }
+}
+
+pub mod binop {
+    use super::*;
+    /// binop::mul_mat_same_storage (binop.rs:115-130): element-wise product; mixed storage
+    /// panics "Storage mismatch" (no conversion).
+    pub fn mul_mat_same_storage<I: SpIndex, Iptr: SpIndex>(lhs: &DeviceCsMat<I, Iptr>, rhs: &DeviceCsMat<I, Iptr>) -> CsMatI<f64, I, Iptr> {
+        super::csmat_binop(lhs, rhs, ffi::SPRS_B200_BINOP_MUL)
+    }
 }
 
 /// sprs::linalg::bicgstab::BiCGSTAB<f64> (linalg/bicgstab.rs:95-300) with x, r, rhat, p

@@ -7,10 +7,10 @@ creating a Context without one raises ThirdPartyError.
 """
 from . import _lib, io, linalg
 from .sparse import (CSC, CSR, Context, CsMat, CsVec, DeviceCsMat, SprsPanic, ThirdPartyError,
-                     csmat_mul_csmat, prod, smmp)
+                     binop, csmat_mul_csmat, prod, smmp)
 
 __all__ = ["CSC", "CSR", "Context", "CsMat", "CsVec", "DeviceCsMat", "SprsPanic",
-           "ThirdPartyError", "csmat_mul_csmat", "prod", "smmp", "_lib", "io", "linalg"]
+           "ThirdPartyError", "binop", "csmat_mul_csmat", "prod", "smmp", "_lib", "io", "linalg"]
 __version__ = "0.1.0"
 import os as _os
 
@@ -45,3 +45,49 @@ def spmv_rows_cut_by_tiles(indptr, tiles=False):
     tile_row = np.concatenate([[0], r, [rows]]).astype(np.int64)
     tile_k = np.concatenate([[0], k, [int(ip[-1])]]).astype(np.int64)
     return cut, tile_row, tile_k
+
+
+BINOP_TILE = 1024      # cost units per binop warp tile (csrc/binop.cu)
+BINOP_LANE_COST = 32   # cost units per lane of a tile
+BINOP_ROW_COST = 16    # cost of one outer dimension's end
+
+
+def binop_cuts(a, b, d):
+    """The binop's merge-path cuts (csrc/binop.cu cut_at restated in numpy, one cut per entry
+    of the cost positions d): a, b = (indptr, indices) of the two operands.  Returns (r, ka, kb)
+    int64 arrays: rows passed and entries of A / B consumed, the split snapped so that an equal
+    pair A[ka-1] == B[kb] is never separated.  `snapped` (4th array) marks the cuts the snap
+    moved.  Tests use it to assert that a matrix puts a cut where they want one."""
+    import numpy as np
+    ipa = np.asarray(a[0]).astype(np.int64)
+    ipb = np.asarray(b[0]).astype(np.int64)
+    ia, ib = np.asarray(a[1]).astype(np.int64), np.asarray(b[1]).astype(np.int64)
+    outer = len(ipa) - 1
+    w = ipa + ipb + BINOP_ROW_COST * np.arange(outer + 1)
+    d = np.asarray(d, dtype=np.int64)
+    r = np.searchsorted(w, d, side="right") - 1
+    ka, kb, snapped = ipa[r].copy(), ipb[r].copy(), np.zeros(d.size, dtype=bool)
+    for i in np.flatnonzero(r < outer):
+        ri = r[i]
+        ra, rb = ia[ipa[ri]:ipa[ri + 1]], ib[ipb[ri]:ipb[ri + 1]]
+        k = min(int(d[i] - w[ri]), len(ra) + len(rb))
+        # ja = A entries among the first k of the stable merge, A first on equal indices
+        order = np.argsort(np.concatenate([ra * 2, rb * 2 + 1]), kind="stable")
+        ja = int(np.count_nonzero(order[:k] < len(ra)))
+        jb = k - ja
+        if ja > 0 and jb < len(rb) and ra[ja - 1] == rb[jb]:
+            jb += 1
+            snapped[i] = True
+        ka[i], kb[i] = ipa[ri] + ja, ipb[ri] + jb
+    return r, ka, kb, snapped
+
+
+def binop_tiles(a, b):
+    """Every tile and lane boundary of the binop on (a, b): the cost positions (tile t starts at
+    t * BINOP_TILE, lane l of it BINOP_LANE_COST * l later, the end of the path last) and their
+    cuts (binop_cuts)."""
+    import numpy as np
+    outer = len(a[0]) - 1
+    total = int(a[0][-1] - a[0][0]) + int(b[0][-1] - b[0][0]) + BINOP_ROW_COST * outer
+    d = np.concatenate([np.arange(0, total, BINOP_LANE_COST, dtype=np.int64), [total]])
+    return (d,) + binop_cuts(a, b, d)

@@ -10,6 +10,7 @@ LIB_PATH = os.path.join(_HERE, "libsprs_b200.so")
 OK, ERR_DIMENSION, ERR_STORAGE, ERR_CUDA, ERR_NCCL, ERR_INDEX_RANGE, ERR_ARGUMENT, \
     ERR_STRUCTURE, ERR_UNSUPPORTED = range(9)
 CSR, CSC = 0, 1
+BINOP_ADD, BINOP_SUB, BINOP_MUL = 0, 1, 2
 
 _vp, _u64, _i64, _int, _dp = C.c_void_p, C.c_uint64, C.c_int64, C.c_int, C.c_void_p
 _dense_sig = [_vp, _vp, _dp, _u64, _u64, _i64, _i64, _dp, _u64, _u64, _i64, _i64]
@@ -44,6 +45,8 @@ PROTOTYPES = {
                                                  C.POINTER(_vp)]),
     "sprs_b200_csmat_check_structure": (_int, [_vp, _vp, C.POINTER(_u64)]),
     "sprs_b200_csmat_to_other_storage": (_int, [_vp, _vp, C.POINTER(_vp)]),
+    "sprs_b200_csmat_binop": (_int, [_vp, _vp, _vp, _int, C.POINTER(_vp)]),
+    "sprs_b200_csmat_scale": (_int, [_vp, _vp, C.c_double, C.POINTER(_vp)]),
     "sprs_b200_mul_acc_mat_vec_csr": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
     "sprs_b200_mul_acc_mat_vec_csc": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
     "sprs_b200_mul_mat_vec": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
@@ -113,7 +116,9 @@ PROTOTYPES = {
 }
 
 _NOT_EMULATED = ("sprs_b200_comm_", "sprs_b200_symm_", "sprs_b200_partition_rows",
-                 "sprs_b200_spmv_rowpart", "sprs_b200_mul_mat_vec_rowpart", "sprs_b200_diag_")
+                 "sprs_b200_spmv_rowpart", "sprs_b200_mul_mat_vec_rowpart", "sprs_b200_diag_",
+                 # the binops are in a separate emulated build (tests/emu_binop.py)
+                 "sprs_b200_csmat_binop", "sprs_b200_csmat_scale")
 _lib = None
 
 

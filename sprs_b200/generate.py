@@ -225,13 +225,18 @@ def spgemm(ctx, a, b):
         ctx.check(lib.sprs_b200_spgemm_numeric_dev(ctx.h, plan, C.byref(cm)))
     finally:
         lib.sprs_b200_spgemm_free(plan)
-    mirror = DeviceCsMat(ctx, cm)
+    return _with_views(ctx, DeviceCsMat(ctx, cm))
+
+
+def _with_views(ctx, mirror):
+    """(mirror, indptr, indices, data): zero-copy torch views of a result mirror's arrays."""
     d_ip, d_ind, d_dat, ipb = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int()
-    ctx.check(lib.sprs_b200_csmat_device_arrays(cm, C.byref(d_ip), C.byref(ipb), C.byref(d_ind),
-                                                C.byref(d_dat)))
+    ctx.check(ctx.lib.sprs_b200_csmat_device_arrays(mirror.h, C.byref(d_ip), C.byref(ipb),
+                                                    C.byref(d_ind), C.byref(d_dat)))
     dev = _device(ctx)
-    rows, nnz = mirror.rows, int(nnz_c.value)
-    indptr = torch.as_tensor(_DevArray(d_ip.value, rows + 1, "<i4" if ipb.value == 4 else "<i8"),
+    outer = mirror.rows if mirror.storage == "CSR" else mirror.cols
+    nnz = mirror.nnz
+    indptr = torch.as_tensor(_DevArray(d_ip.value, outer + 1, "<i4" if ipb.value == 4 else "<i8"),
                              device=dev)
     if nnz:
         indices = torch.as_tensor(_DevArray(d_ind.value, nnz, "<i4"), device=dev)
@@ -240,3 +245,30 @@ def spgemm(ctx, a, b):
         indices = torch.empty(0, dtype=torch.int32, device=dev)
         data = torch.empty(0, dtype=torch.float64, device=dev)
     return mirror, indptr, indices, data
+
+
+_BINOP_OPS = {"add": _lib.BINOP_ADD, "sub": _lib.BINOP_SUB, "mul": _lib.BINOP_MUL}
+
+
+def binop(ctx, a, b, op):
+    """C = A + B ("add"), A - B ("sub") or A .* B ("mul") on the device (csmat_binop,
+    binop.rs:178-271; same storage and shape).  Returns (mirror, indptr, indices, data) like
+    spgemm: the DeviceCsMat that owns C and zero-copy torch views of its arrays."""
+    ma = a.mirror if isinstance(a, DeviceCsr) else a
+    mb = b.mirror if isinstance(b, DeviceCsr) else b
+    if _device(ctx).type == "cuda":
+        _sync()  # operands produced on torch's stream; the binop runs on the ctx stream
+    cm = C.c_void_p()
+    ctx.check(ctx.lib.sprs_b200_csmat_binop(ctx.h, ma.h, mb.h, _BINOP_OPS[op], C.byref(cm)))
+    return _with_views(ctx, DeviceCsMat(ctx, cm))
+
+
+def scale(ctx, a, s):
+    """C = A * s on the device (CsMatBase::map: same structure, zeros kept); returns
+    (mirror, indptr, indices, data) like binop."""
+    ma = a.mirror if isinstance(a, DeviceCsr) else a
+    if _device(ctx).type == "cuda":
+        _sync()
+    cm = C.c_void_p()
+    ctx.check(ctx.lib.sprs_b200_csmat_scale(ctx.h, ma.h, float(s), C.byref(cm)))
+    return _with_views(ctx, DeviceCsMat(ctx, cm))

@@ -10,6 +10,8 @@ reference's own tests.  Same names, argument meaning and error behaviour:
                                       sprs/src/sparse/vec.rs:1084-1131
   prod.mul_acc_mat_vec_csr, ...       sprs/src/sparse/prod.rs
   smmp.mul_csr_csr, symbolic+numeric  sprs/src/sparse/smmp.rs
+  a + b, a - b, a * s                 `impl Add/Sub/Mul<N>` sprs/src/sparse/binop.rs:20-163
+  binop.mul_mat_same_storage          sprs/src/sparse/binop.rs:115-130
 
 Contract violations raise SprsPanic with the reference's panic message
 ("Dimension mismatch", "Storage mismatch"; sprs Guidelines.rst:9-27); device
@@ -444,12 +446,28 @@ class CsMat:
                 return _csmat_mul_dense_vec(self, rhs)
             if rhs.ndim == 2:
                 return _csmat_mul_dense_mat(self, rhs)
+        if isinstance(rhs, (float, int, np.floating, np.integer)):
+            return _csmat_scale(self, float(rhs))
         return NotImplemented
 
     __matmul__ = __mul__
 
     def dot(self, rhs):
         return self.__mul__(rhs)
+
+    # -- `impl Add` / `impl Sub` / `impl Mul<N>` of binop.rs:20-163
+    def __add__(self, rhs):
+        """`&A + &B` (binop.rs:20-65): a new matrix in lhs storage; rhs converted with
+        to_other_storage when the storages differ; entries whose sum is 0.0 are dropped."""
+        if isinstance(rhs, CsMat):
+            return _csmat_binop_other_storage(self, rhs, _lib.BINOP_ADD)
+        return NotImplemented
+
+    def __sub__(self, rhs):
+        """`&A - &B` (binop.rs:67-112), same rules as `+`."""
+        if isinstance(rhs, CsMat):
+            return _csmat_binop_other_storage(self, rhs, _lib.BINOP_SUB)
+        return NotImplemented
 
     def __rmatmul__(self, lhs):
         """dense.dot(&sparse) = (sparse^T . dense^T)^T  (csmat.rs:2050-2099)."""
@@ -459,6 +477,56 @@ class CsMat:
 
 
 # ------------------------------------------------------------------------------------
+def _new_trusted_like(lhs, dev):
+    """The CsMat of a device result in lhs's storage, shape and index dtypes (new_trusted,
+    binop.rs:210-217); the result's mirror stays attached for the next device operation."""
+    ip, ind, dat = dev.download(lhs.indices.dtype, lhs.indptr.dtype)
+    out = object.__new__(CsMat)
+    out.storage, out.shape = lhs.storage, lhs.shape
+    out.indptr, out.indices, out.data = ip, ind, dat
+    out._ctx, out._dev = lhs._ctx, dev
+    return out
+
+
+def _csmat_binop(lhs, rhs_dev, op):
+    """csmat_binop (binop.rs:178-271) on the device: lhs a CsMat, rhs a mirror of the same
+    storage.  The reference asserts the shapes first, then the storage."""
+    ctx = lhs.context()
+    out = C.c_void_p()
+    ctx.check(ctx.lib.sprs_b200_csmat_binop(ctx.h, lhs.device().h, rhs_dev.h, op, C.byref(out)))
+    return _new_trusted_like(lhs, DeviceCsMat(ctx, out))
+
+
+def _csmat_binop_other_storage(lhs, rhs, op):
+    """Add / Sub (binop.rs:20-112): shapes checked, then rhs converted to lhs's storage."""
+    if lhs.shape != rhs.shape:
+        raise SprsPanic("Dimension mismatch")
+    rhs_dev = rhs.device() if rhs.storage == lhs.storage else rhs.device().to_other_storage()
+    return _csmat_binop(lhs, rhs_dev, op)
+
+
+# `impl Mul<N> for &CsMatBase` binop.rs:132-163 -> CsMatBase::map (csmat.rs:1289-1305)
+def _csmat_scale(a, s):
+    ctx = a.context()
+    out = C.c_void_p()
+    ctx.check(ctx.lib.sprs_b200_csmat_scale(ctx.h, a.device().h, s, C.byref(out)))
+    return _new_trusted_like(a, DeviceCsMat(ctx, out))
+
+
+class binop:
+    """Free functions of sprs/src/sparse/binop.rs."""
+
+    @staticmethod
+    def mul_mat_same_storage(lhs, rhs):
+        """binop.rs:115-130: element-wise (Hadamard) product of two matrices of the same shape
+        AND storage -- no conversion: mixed storage panics "Storage mismatch"."""
+        if lhs.shape != rhs.shape:
+            raise SprsPanic("Dimension mismatch")
+        if lhs.storage != rhs.storage:
+            raise SprsPanic("Storage mismatch")
+        return _csmat_binop(lhs, rhs.device(), _lib.BINOP_MUL)
+
+
 # `impl Mul<&ArrayBase<_, Ix1>> for &CsMatBase`  csmat.rs:2119-2160
 def _csmat_mul_dense_vec(a, x):
     if a.cols() != x.shape[0]:

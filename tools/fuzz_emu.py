@@ -31,7 +31,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import exact  # noqa: E402  (tests/exact.py: integer-valued inputs)
 
 
-def setup(schedule):
+def setup(schedule, binop=False):
     os.environ["SPRS_B200_EMU"] = "1"
     if schedule:
         os.environ["CUEMU_SCHEDULE"] = schedule
@@ -39,7 +39,11 @@ def setup(schedule):
     import sprs_b200
     from conftest import emu_library
     from sprs_b200 import generate
-    sprs_b200._lib.LIB_PATH = emu_library()
+    if binop:  # the emulated build with csrc/binop.cu (tests/emu_binop.py)
+        from emu_binop import emu_binop_library
+        sprs_b200._lib.LIB_PATH = emu_binop_library()
+    else:
+        sprs_b200._lib.LIB_PATH = emu_library()
     generate._device = lambda ctx: torch.device("cpu")
     generate._stream_ptr = lambda: None
     generate._sync = lambda: None
@@ -339,20 +343,63 @@ def one_case(sp, O, seed):
     return errs
 
 
+BINOP_LENS = [0, 0, 1, 2, 15, 16, 17, 31, 32, 33, 63, 64, 65, 1007, 1008, 1023, 1024, 1025, 3000]
+
+
+def binop_case(sp, O, seed):
+    """--binop: `+`, `-`, mul_mat_same_storage and `* s` (csrc/binop.cu) against the binop oracle,
+    bit for bit (NaN by class).  Row lengths sit on the tile (1024 cost units, a row end 16),
+    lane (32 units) and snap boundaries; B overlaps A (forced equal pairs) or cancels it."""
+    import binop_oracle as BO
+    rng = np.random.default_rng(seed)
+    rows, cols = int(rng.integers(0, 160)), int(rng.integers(1, 4000))
+    la = np.minimum(rng.choice(BINOP_LENS, rows), cols)
+    a = make_csr(rng, rows, cols, la, integer=bool(seed & 1))
+    mode = rng.integers(0, 3)
+    if mode == 0:    # independent patterns
+        b = make_csr(rng, rows, cols, np.minimum(rng.choice(BINOP_LENS, rows), cols))
+    else:            # A's pattern, thinned: equal pairs everywhere, exact cancellations (mode 2)
+        keep = rng.random(a[1].size) < 0.7
+        r_of = np.repeat(np.arange(rows), np.diff(a[0].astype(np.int64)))
+        ip = np.zeros(rows + 1, np.int64)
+        np.cumsum(np.bincount(r_of[keep], minlength=rows), out=ip[1:])
+        d = a[2][keep] if mode == 2 else rng.standard_normal(int(keep.sum()))
+        b = (ip.astype(np.uint32), a[1][keep], d)
+    A, B = sp.CsMat.new((rows, cols), *a), sp.CsMat.new((rows, cols), *b)
+    if rng.random() < 0.25:  # CSC + CSC
+        A, B = A.to_other_storage(), B.to_other_storage()
+    errs = []
+    cast = lambda m: (m.indptr.astype(np.uint64), m.indices.astype(np.uint32), m.data)  # noqa: E731
+    ops = [(BO.ADD, lambda: A + B), (BO.SUB, lambda: A - B),
+           (BO.MUL, lambda: sp.binop.mul_mat_same_storage(A, B))]
+    for op, f in [ops[i] for i in rng.permutation(3)]:
+        got = f()
+        e = BO.first_difference((got.indptr, got.indices, got.data), BO.binop(op, cast(A), cast(B)))
+        if e:
+            errs.append("binop %d: %s" % (op, e))
+    s = float(rng.choice([2.0, -0.5, 0.0, np.inf]))
+    got = A * s
+    e = BO.first_difference((got.indptr, got.indices, got.data), BO.scale(cast(A), s))
+    if e:
+        errs.append("scale: " + e)
+    return errs
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seconds", type=float, default=120)
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--schedule", default="")
     ap.add_argument("--cases", type=int, default=0)
+    ap.add_argument("--binop", action="store_true", help="fuzz the sparse binops instead")
     args = ap.parse_args()
-    sp, O = setup(args.schedule)
+    sp, O = setup(args.schedule, args.binop)
     t0 = time.time()
     n = fails = 0
     seed = args.seed
     while (args.cases and n < args.cases) or (not args.cases and time.time() - t0 < args.seconds):
         try:
-            errs = one_case(sp, O, seed)
+            errs = (binop_case if args.binop else one_case)(sp, O, seed)
         except Exception as e:  # a panic / status code where none is expected is a finding too
             errs = ["exception %s: %s" % (type(e).__name__, e)]
         for e in errs:
