@@ -221,7 +221,11 @@ int sprs_b200_copy_to_device(sprs_b200_ctx* ctx, void* d_dst, const void* h_src,
 int sprs_b200_copy_to_host(sprs_b200_ctx* ctx, void* h_dst, const void* d_src, uint64_t bytes,
                            void* stream);
 /* all-gather "put": copy y[row_offset .. row_offset+rows) of this rank's buffer into the same
- * position of n_peers peer buffers with one kernel (coalesced stores over NVLink).        */
+ * position of n_peers (0..8) peer buffers with one kernel (coalesced 16-byte stores over
+ * NVLink).  Every peer buffer must be non-null and have the same address modulo 16 as
+ * d_y_own (any two cudaMalloc / symm_alloc buffers do), else ERR_ARGUMENT and nothing is
+ * launched.  The same rule holds for d_y_bufs[1..) against d_y_bufs[0] in
+ * spmv_chunked_push_dev.                                                                  */
 int sprs_b200_peer_push_dev(sprs_b200_ctx* ctx, const double* d_y_own, uint64_t row_offset,
                             uint64_t rows, int n_peers, double* const* d_y_peers, void* stream);
 int sprs_b200_spmv_allgather_dev(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat,

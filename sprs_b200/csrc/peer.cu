@@ -44,14 +44,36 @@ __global__ void __launch_bounds__(256)
             for (int q = 0; q < dst.n; ++q) dst.p[q][count - 1] = src[count - 1];
     }
 }
+
+// The put kernel takes its scalar head from the source address alone and stores double2 through
+// every target, so each target must be non-null and share the source's 16-byte parity.
+int check_push_targets(sprs_b200_ctx* ctx, const double* src, const SpmvTargets& dst) {
+    for (int q = 0; q < dst.n; ++q) {
+        if (!dst.p[q]) SPRS_FAIL(ctx, SPRS_B200_ERR_ARGUMENT, "peer push: target %d is null", q);
+        if ((((uintptr_t)dst.p[q]) & 15) != (((uintptr_t)src) & 15))
+            SPRS_FAIL(ctx, SPRS_B200_ERR_ARGUMENT, "peer push: buffers must share their 16-byte alignment");
+    }
+    return SPRS_B200_OK;
+}
+
+// dst = bufs[0 .. n) + offset, checked against the put's source `src` (the same offset into the
+// rank's own buffer).  A null buffer is caught before the offset makes it look valid.
+int push_targets(sprs_b200_ctx* ctx, const double* src, double* const* bufs, int n, uint64_t offset,
+                 SpmvTargets* dst) {
+    dst->n = n;
+    for (int q = 0; q < SPMV_MAX_TARGETS; ++q) {
+        if (q < n && !bufs[q]) SPRS_FAIL(ctx, SPRS_B200_ERR_ARGUMENT, "peer push: target %d is null", q);
+        dst->p[q] = q < n ? bufs[q] + offset : nullptr;
+    }
+    return check_push_targets(ctx, src, *dst);
+}
 }  // namespace
 
 int peer_push_launch(sprs_b200_ctx* ctx, const double* src, const SpmvTargets& dst, uint64_t count,
                      cudaStream_t s) {
-    if (count == 0 || dst.n == 0) return SPRS_B200_OK;
-    for (int q = 0; q < dst.n; ++q)
-        if ((((uintptr_t)dst.p[q]) & 15) != (((uintptr_t)src) & 15))
-            SPRS_FAIL(ctx, SPRS_B200_ERR_ARGUMENT, "peer push: buffers must share their 16-byte alignment");
+    if (dst.n == 0) return SPRS_B200_OK;
+    SPRS_TRY(check_push_targets(ctx, src, dst));
+    if (count == 0) return SPRS_B200_OK;
     uint64_t blocks = (count / 2 + 1023) / 1024;
     if (blocks == 0) blocks = 1;
     const uint64_t cap = (uint64_t)ctx->sm_count * 2;
@@ -70,9 +92,7 @@ int sprs_b200_peer_push_dev(sprs_b200_ctx* ctx, const double* d_y_own, uint64_t 
     if (n_peers < 0 || n_peers > SPMV_MAX_TARGETS)
         SPRS_FAIL(ctx, SPRS_B200_ERR_ARGUMENT, "n_peers must be 0..%d", SPMV_MAX_TARGETS);
     SpmvTargets dst;
-    dst.n = n_peers;
-    for (int q = 0; q < SPMV_MAX_TARGETS; ++q)
-        dst.p[q] = q < n_peers ? d_y_peers[q] + row_offset : nullptr;
+    SPRS_TRY(push_targets(ctx, d_y_own + row_offset, d_y_peers, n_peers, row_offset, &dst));
     return peer_push_launch(ctx, d_y_own + row_offset, dst, rows, (cudaStream_t)stream);
 }
 
@@ -165,11 +185,16 @@ int sprs_b200_spmv_chunked_push_dev(sprs_b200_ctx* ctx, const sprs_b200_csmat* m
     if (!ctx || !mat || !d_y_bufs) return SPRS_B200_ERR_ARGUMENT;
     if (n_targets < 1 || n_targets > SPMV_MAX_TARGETS)
         SPRS_FAIL(ctx, SPRS_B200_ERR_ARGUMENT, "n_targets must be 1..%d", SPMV_MAX_TARGETS);
+    if (!d_y_bufs[0]) SPRS_FAIL(ctx, SPRS_B200_ERR_ARGUMENT, "d_y_bufs[0] is null");
+    double* y_own = d_y_bufs[0] + row_offset;
+    // every put of the chunks below reads y_own + r0 and stores to d_y_bufs[q] + row_offset + r0:
+    // one check of the targets at r0 = 0 covers all of them
+    SpmvTargets dst;
+    SPRS_TRY(push_targets(ctx, y_own, d_y_bufs + 1, n_targets - 1, row_offset, &dst));
     if (mat->storage != SPRS_B200_CSR)
         SPRS_FAIL(ctx, SPRS_B200_ERR_STORAGE, "Storage mismatch: spmv needs a CSR mirror");
     if (mat->rows == 0) return SPRS_B200_OK;
     cudaStream_t s = (cudaStream_t)stream;
-    double* y_own = d_y_bufs[0] + row_offset;
     if (n_chunks <= 0) n_chunks = 4;
     if (const char* e = getenv("SPRS_B200_PUSH_CHUNKS")) n_chunks = atoi(e) > 0 ? atoi(e) : n_chunks;
     if (n_chunks > SPRS_E2E_MAX_CHUNKS) n_chunks = SPRS_E2E_MAX_CHUNKS;
@@ -183,9 +208,6 @@ int sprs_b200_spmv_chunked_push_dev(sprs_b200_ctx* ctx, const sprs_b200_csmat* m
     if (!ctx->ev_chunk[0])
         for (int i = 0; i < SPRS_E2E_MAX_CHUNKS; ++i)
             SPRS_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_chunk[i], cudaEventDisableTiming));
-    SpmvTargets dst;
-    dst.n = n_targets - 1;
-    for (int q = 0; q < SPMV_MAX_TARGETS; ++q) dst.p[q] = nullptr;
     const size_t nc = mat->push_tiles.size() - 1;
     for (size_t c = 0; c < nc; ++c) {
         SPRS_TRY(spmv_launch_tile_range(ctx, mat, d_x, y_own, accumulate, mat->push_tiles[c],

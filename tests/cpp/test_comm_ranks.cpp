@@ -3,8 +3,10 @@
 // SpMV in every exchange mode (device-resident and host-vector forms), device barrier.
 // The ranks use device rank % n_devices, so on a single-GPU box both ranks share device 0 and
 // the whole multi-rank logic still runs on hardware.  Usage: test_comm_ranks [world]
-// Checks: every rank ends with the FULL y = A x (sequential CPU sum of this file, gate
-// |d| <= 1e-6 * sum|terms|, SURVEY 8d) for every exchange mode, twice in a row.
+// Checks: every rank ends with the FULL y = A x for every exchange mode, twice in a row with a
+// different x each time, BIT FOR BIT against the sequential CPU sum of this file.  A and x hold
+// small integers, so every partial sum is exact and every summation order gives the same bits;
+// a row that is dropped, doubled, misplaced or left over from the previous product fails.
 #include <sys/wait.h>
 #include <unistd.h>
 
@@ -36,7 +38,13 @@ static uint64_t splitmix(uint64_t& s) {
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
     return z ^ (z >> 31);
 }
-static double unit(uint64_t& s) { return (double)(splitmix(s) >> 11) * (1.0 / 9007199254740992.0) - 0.5; }
+// a non-zero integer in [-m, m]: |A| <= 8, |x| <= 1024 and rows of at most 5000 non-zeros keep
+// every partial sum below 2^26, far inside the exact range of a double
+static double small_int(uint64_t& s, uint64_t m) {
+    const uint64_t h = splitmix(s);
+    return (double)(h % m + 1) * ((h >> 32) & 1 ? -1.0 : 1.0);
+}
+static bool same_bits(double a, double b) { return memcmp(&a, &b, sizeof a) == 0; }
 
 struct Csr {
     uint64_t rows, cols;
@@ -56,7 +64,7 @@ static Csr make_matrix(uint64_t rows, uint64_t cols, uint64_t seed) {
         uint64_t c = splitmix(s) % (cols / (len + 1) + 1);
         for (uint64_t k = 0; k < len && c < cols; ++k) {
             m.indices.push_back((uint32_t)c);
-            m.data.push_back(unit(s));
+            m.data.push_back(small_int(s, 8));
             c += 1 + splitmix(s) % (2 * cols / (len + 1) + 1) / 2;
         }
         m.indptr.push_back((uint32_t)m.indices.size());
@@ -80,14 +88,16 @@ static int run_rank(int rank, int world, const char* id) {
 
     const uint64_t n = 20000;
     const Csr a = make_matrix(n, n, 0x5EED);
-    std::vector<double> x(n), ref(n, 0.0), bound(n, 0.0);
+    // two x vectors used in turn, so that a stale row of the previous product is wrong
+    std::vector<double> xv[2] = {std::vector<double>(n), std::vector<double>(n)};
+    std::vector<double> ref[2] = {std::vector<double>(n, 0.0), std::vector<double>(n, 0.0)};
     uint64_t s = 77;
-    for (auto& v : x) v = unit(s);
-    for (uint64_t r = 0; r < n; ++r)
-        for (uint32_t k = a.indptr[r]; k < a.indptr[r + 1]; ++k) {
-            ref[r] += a.data[k] * x[a.indices[k]];
-            bound[r] += std::fabs(a.data[k] * x[a.indices[k]]);
-        }
+    for (int v = 0; v < 2; ++v) {
+        for (auto& e : xv[v]) e = small_int(s, 1024);
+        for (uint64_t r = 0; r < n; ++r)
+            for (uint32_t k = a.indptr[r]; k < a.indptr[r + 1]; ++k)
+                ref[v][r] += a.data[k] * xv[v][a.indices[k]];
+    }
     // partition (every rank computes the same cut points) and this rank's block
     std::vector<uint64_t> bounds(world + 1);
     CK(ctx, sprs_b200_partition_rows(a.indptr.data(), 4, n, world, 8.0, bounds.data()));
@@ -108,7 +118,9 @@ static int run_rank(int rank, int world, const char* id) {
     for (int g = 0; g < world; ++g) tot += all_nnz[g];
     if (tot != a.indices.size()) return 6;
 
-    int checks = 0;
+    // a mismatch is reported and remembered, never returned early: the other ranks wait for this
+    // one at every collective call below, so it keeps making them
+    int checks = 0, fail = 0;
     for (int want_mc = 0; want_mc <= 1; ++want_mc) {
         sprs_b200_symm *y = nullptr, *xs = nullptr;
         CK(ctx, sprs_b200_symm_alloc(comm, n * 8, want_mc, &y));
@@ -119,20 +131,20 @@ static int run_rank(int rank, int world, const char* id) {
                    sprs_b200_comm_multicast_supported(comm));
         // device-resident form: x replicated, y all-gathered
         double* d_x = (double*)sprs_b200_symm_ptr(xs, rank);
-        // upload x through the host-vector form first (also tests the x all-gather)
-        std::vector<double> yh(r1 - r0, -1.0);
-        for (int rep = 0; rep < 2; ++rep) {
-            CK(ctx, sprs_b200_mul_mat_vec_rowpart(comm, blk, xs, x.data() + r0, r0, r1 - r0,
-                                                  yh.data(), r1 - r0));
-            for (uint64_t r = r0; r < r1; ++r, ++checks)
-                if (!(std::fabs(yh[r - r0] - ref[r]) <= 1e-6 * bound[r] + 1e-300)) {
-                    fprintf(stderr, "[rank %d] e2e mc=%d row %llu: %g vs %g\n", rank, (int)mc,
-                            (unsigned long long)r, yh[r - r0], ref[r]);
-                    return 7;
-                }
-        }
         for (int mode : {SPRS_B200_EXCHANGE_FUSED, SPRS_B200_EXCHANGE_PUSH, SPRS_B200_EXCHANGE_AUTO}) {
             for (int rep = 0; rep < 2; ++rep) {
+                // the host-vector form uploads this rep's x (also tests the x all-gather); the
+                // device-resident form below then reads the same x from the symmetric buffer
+                std::vector<double> yh(r1 - r0, NAN);
+                CK(ctx, sprs_b200_mul_mat_vec_rowpart(comm, blk, xs, xv[rep].data() + r0, r0, r1 - r0,
+                                                      yh.data(), r1 - r0));
+                for (uint64_t r = r0; r < r1; ++r, ++checks)
+                    if (!same_bits(yh[r - r0], ref[rep][r])) {
+                        fprintf(stderr, "[rank %d] e2e mc=%d rep %d row %llu: %.17g vs %.17g\n", rank,
+                                (int)mc, rep, (unsigned long long)r, yh[r - r0], ref[rep][r]);
+                        fail = 7;
+                        break;
+                    }
                 // poison this rank's y so that a row that never arrives is caught
                 std::vector<double> poison(n, NAN), got(n);
                 CK(ctx, sprs_b200_comm_barrier_dev(comm, nullptr));
@@ -143,10 +155,11 @@ static int run_rank(int rank, int world, const char* id) {
                 CK(ctx, sprs_b200_comm_check(comm, nullptr));
                 CK(ctx, sprs_b200_copy_to_host(ctx, got.data(), sprs_b200_symm_ptr(y, rank), n * 8, nullptr));
                 for (uint64_t r = 0; r < n; ++r, ++checks)
-                    if (!(std::fabs(got[r] - ref[r]) <= 1e-6 * bound[r] + 1e-300)) {
-                        fprintf(stderr, "[rank %d] mode %d mc=%d rep %d row %llu: %g vs %g\n", rank,
-                                mode, (int)mc, rep, (unsigned long long)r, got[r], ref[r]);
-                        return 9;
+                    if (!same_bits(got[r], ref[rep][r])) {
+                        fprintf(stderr, "[rank %d] mode %d mc=%d rep %d row %llu: %.17g vs %.17g\n", rank,
+                                mode, (int)mc, rep, (unsigned long long)r, got[r], ref[rep][r]);
+                        fail = 9;
+                        break;
                     }
             }
         }
@@ -156,6 +169,7 @@ static int run_rank(int rank, int world, const char* id) {
     sprs_b200_csmat_free(blk);
     CK(ctx, sprs_b200_comm_free(comm));
     sprs_b200_ctx_destroy(ctx);
+    if (fail) return fail;
     if (rank == 0) printf("OK %d checks per rank, world %d\n", checks, world);
     return 0;
 }
