@@ -15,7 +15,8 @@
 //     is L1 for the gathers);
 //   * ROWS STRAIGHT FROM GLOBAL MEMORY, lanes matched to the rows (rows_direct): per block of 31
 //     rows, tiny rows (<= 8 non-zeros) one lane each in storage order -- the reference's bits
-//     --, the others packed G = 4..32 lanes per row with 4 index / value / gather loads in
+//     where no tile carries the row, from y[r] when accumulating --, the others packed G = 4..32
+//     lanes per row with 4 index / value / gather loads in
 //     flight per lane and one G-lane butterfly per row, very long rows by the whole warp.
 //     Nothing is staged, nothing but a row sum crosses lanes;
 //   * loads: ld.global.nc.L1::no_allocate + L2 evict_first for the matrix (read exactly once),
@@ -29,7 +30,9 @@
 //   * HOT SET (large skewed matrices, spmv_prepare_hot): x of the K most-referenced columns is
 //     staged in shared memory by every CTA (one 32-warp CTA per SM) and the kernel reads a
 //     tagged copy of the index stream, so those gathers move no L2 sector.
-// Rows longer than 8 non-zeros use trees and agree with the reference to rounding (parity gate:
+// The summation order depends only on indptr and the cut constants, and y is bit-identical to
+// tests/spmv_model.py (its host restatement) for any values.  Rows longer than 8 non-zeros and
+// carried rows (y0 + partial + carries) agree with the reference to rounding (parity gate:
 // |d| <= 1e-6 * sum|terms|, SURVEY 8d).  Arithmetic is MulAcc::mul_acc's (mul_acc.rs:28-30):
 // unfused multiply, then add.
 //
@@ -42,6 +45,7 @@
 
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 namespace {
 
@@ -101,10 +105,11 @@ struct RowSink {
 // peer GPUs' y buffers (CUDA IPC / VMM mappings) or the NVSwitch multicast address of y (fused
 // SpMV + all-gather over NVLink: the result of a row leaves for the peers the moment it is
 // reduced, overlapped with the rest of the kernel, instead of a separate collective afterwards).
+// from_y: the sum already started from y[r] (tiny rows under accumulate), so it is stored as is.
 template <bool MULTI>
-__device__ __forceinline__ void sink_row(const RowSink& k, uint64_t r, double sum) {
+__device__ __forceinline__ void sink_row(const RowSink& k, uint64_t r, double sum, bool from_y = false) {
     if (r < k.r1) {
-        const double v = k.accumulate ? __dadd_rn(k.y[r], sum) : sum;
+        const double v = k.accumulate && !from_y ? __dadd_rn(k.y[r], sum) : sum;
         k.y[r] = v;
         if (MULTI) {
 #pragma unroll
@@ -140,7 +145,8 @@ __device__ __forceinline__ double gather_x(const double* __restrict__ x, const d
 // of 31 rows is taken in three sweeps, because R-MAT blocks mix rows of 0, 5, 50 and 5000
 // non-zeros and any single lanes-per-row choice leaves most lanes idle:
 //   1. TINY rows (at most 2U = 8 non-zeros, empty rows included): every lane takes its own row,
-//      all of them in one pass, summed in storage order -- the reference's bits for every such row;
+//      all of them in one pass, summed in storage order (from y[r] when accumulating a row that
+//      no tile carries: the reference's bits);
 //   2. the other rows, packed (no slot is spent on a tiny row): G lanes per row, 32/G rows per
 //      pass, each group walking its row with stride G; one G-lane butterfly finishes a row;
 //   3. rows longer than 4 steps of their group: the whole warp, one row at a time.
@@ -169,32 +175,44 @@ __device__ __forceinline__ void rows_direct(const RowSink& k, const P* __restric
         me = me < k1 ? me : k1;
         if (lane >= nrows || me < ms) me = ms;
         const bool tiny = lane < nrows && (me - ms) <= (P)(2 * U);
-        // ---- sweep 1: tiny rows, one lane each, storage order
-        if (__any_sync(FULL, tiny && me > ms)) {
-            double acc = 0.0;
+        // ---- sweep 1: tiny rows, one lane each, storage order.  Accumulating, a row that no tile
+        // carries starts from y[r] -- ((y0 + p0) + p1) + ..., the reference's order -- and an empty
+        // one keeps y's bits (-0.0 included).  Row r0 is the previous tile's carry row, except in
+        // tile 0, the only tile that starts at (row 0, non-zero 0).
+        // (accumulate is uniform: each form gets its own copy of the sweep, so the plain one has
+        // no y load and keeps its 48 registers)
+        const uint32_t rl = rbase + lane;
+        auto tiny_sweep = [&](auto acc_tag) {
+            constexpr bool ACC = decltype(acc_tag)::value;
+            const bool from_y = ACC && tiny && rl < k.r1 && (rl > r0 || (r0 == 0 && k0 == 0));
+            double acc = from_y ? k.y[rl] : 0.0;  // (empty rows: y = 0, or y + 0 for a carried row)
+            if (__any_sync(FULL, tiny && me > ms)) {
 #pragma unroll
-            for (int st = 0; st < 2; ++st) {
-                const P q = ms + (P)(st * U);
-                uint32_t c[U];
-                double v[U], xv[U];
+                for (int st = 0; st < 2; ++st) {
+                    const P q = ms + (P)(st * U);
+                    uint32_t c[U];
+                    double v[U], xv[U];
 #pragma unroll
-                for (int u = 0; u < U; ++u)
-                    c[u] = (tiny && q + (P)u < me) ? ldg_stream_u32(indices + q + (P)u, pol_stream) : 0u;
+                    for (int u = 0; u < U; ++u)
+                        c[u] = (tiny && q + (P)u < me) ? ldg_stream_u32(indices + q + (P)u, pol_stream) : 0u;
 #pragma unroll
-                for (int u = 0; u < U; ++u)
-                    v[u] = (tiny && q + (P)u < me) ? ldg_stream_f64(data + q + (P)u, pol_stream) : 0.0;
+                    for (int u = 0; u < U; ++u)
+                        v[u] = (tiny && q + (P)u < me) ? ldg_stream_f64(data + q + (P)u, pol_stream) : 0.0;
 #pragma unroll
-                for (int u = 0; u < U; ++u)
-                    xv[u] = (tiny && q + (P)u < me) ? gather_x<HOT>(x, hot, c[u], polx) : 0.0;
+                    for (int u = 0; u < U; ++u)
+                        xv[u] = (tiny && q + (P)u < me) ? gather_x<HOT>(x, hot, c[u], polx) : 0.0;
 #pragma unroll
-                for (int u = 0; u < U; ++u)
-                    if (tiny && q + (P)u < me) acc = __dadd_rn(acc, __dmul_rn(v[u], xv[u]));
-                if (!__any_sync(FULL, tiny && q + (P)U < me)) break;
+                    for (int u = 0; u < U; ++u)
+                        if (tiny && q + (P)u < me) acc = __dadd_rn(acc, __dmul_rn(v[u], xv[u]));
+                    if (!__any_sync(FULL, tiny && q + (P)U < me)) break;
+                }
             }
-            if (tiny) sink_row<MULTI>(k, (uint64_t)rbase + lane, acc);
-        } else if (tiny) {
-            sink_row<MULTI>(k, (uint64_t)rbase + lane, 0.0);  // empty rows: y = 0 (or y += 0)
-        }
+            if (tiny) sink_row<MULTI>(k, (uint64_t)rbase + lane, acc, from_y);
+        };
+        if (k.accumulate)
+            tiny_sweep(std::true_type{});
+        else
+            tiny_sweep(std::false_type{});
         // ---- sweeps 2 and 3: the other rows, NG at a time
         unsigned todo = __ballot_sync(FULL, lane < nrows && !tiny);
         while (todo) {

@@ -5,9 +5,10 @@ The algebra is that of the reference, one rounding per operation: every product 
 or difference is its own numpy operation (numpy never fuses them), and the scalar algebra is done
 on float64 scalars in the reference's order.  Two parts are plug-ins:
 
-  matvec   y = A x for a fresh y: `oracle_matvec` (the oracle's sequential row sums) or
+  matvec   y = A x for a fresh y: `oracle_matvec` (the oracle's sequential row sums),
            `device_matvec` (the library's sprs_b200_spmv_dev on a device mirror -- the entry the
-           solver's own SpMV calls, so it gives the same bits for the same mirror).
+           solver's own SpMV calls, so it gives the same bits for the same mirror) or
+           `model_matvec` (the SpMV's order restated on the host, tests/spmv_model.py).
   reduce   the sum of a vector of products: `sequential` (+0.0 + t0 + t1 + ..., vec.rs:846-881,
            907-913, the oracle's order) or `device(grid)`, the order of csrc/solver.cu:
              * thread t of the grid's grid * 256 threads visits chunks t, t + grid*256, ... of 4
@@ -135,6 +136,12 @@ def oracle_matvec(O, indptr, indices, data):
     """y = A x with the oracle's row sums (prod.rs:103-127 into a zero vector)."""
     rows = len(indptr) - 1
     return lambda x: O.mul_acc_mat_vec_csr(indptr, indices, data, x, np.zeros(rows))
+
+
+def model_matvec(indptr, indices, data):
+    """y = A x in the device SpMV's order, restated on the host (tests/spmv_model.py)."""
+    import spmv_model
+    return lambda x: spmv_model.spmv(indptr, indices, data, x)
 
 
 def device_matvec(ctx, mirror):
