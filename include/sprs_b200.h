@@ -52,7 +52,9 @@ enum {
     SPRS_B200_ERR_ARGUMENT = 6,    /* null pointer, bad width, bad handle                */
     SPRS_B200_ERR_STRUCTURE = 7,   /* indptr not monotone / index out of bounds          */
     SPRS_B200_ERR_UNSUPPORTED = 8,
-    SPRS_B200_ERR_COMM = 9         /* multi-GPU rendezvous / barrier failure; see last_error */
+    SPRS_B200_ERR_COMM = 9,        /* multi-GPU rendezvous / barrier failure; see last_error */
+    SPRS_B200_ERR_SINGULAR = 10    /* LinalgError::SingularMatrix (errors.rs:59-69); see
+                                      sprs_b200_trisolve_singular                           */
 };
 
 int sprs_b200_version(void);
@@ -392,6 +394,48 @@ int sprs_b200_bicgstab_stats(const sprs_b200_bicgstab* s, uint64_t counts[3],
 int sprs_b200_bicgstab_get(const sprs_b200_bicgstab* s, int which, double* out, uint64_t len);
 /* borrowed device pointer to vector `which` (valid until bicgstab_free) */
 int sprs_b200_bicgstab_get_dev(const sprs_b200_bicgstab* s, int which, const double** d_out);
+
+/* ---- sparse triangular solves with a dense right-hand side (sprs::linalg::trisolve,
+ * linalg/trisolve.rs): lsolve_csr_dense_rhs (:30-73), usolve_csr_dense_rhs (:219-262),
+ * lsolve_csc_dense_rhs (:85-149), usolve_csc_dense_rhs (:161-210).  Entries of the other
+ * triangle are ignored.  Every row is x_r = b_r, x_r = x_r - a_rc * x_c over its terms in the
+ * reference's order (ascending column; descending for usolve_csc), then x_r / diag, each
+ * operation rounded on its own: the result is bit-identical to the reference.
+ * A plan is built once per matrix and triangle: it finds every row's diagonal and the first
+ * singular row or column in processing order (diagonal missing or == 0; -0.0 counts as zero,
+ * NaN does not).  The plan BORROWS the mirror and READS ITS VALUES when it is built: the
+ * mirror must be kept alive and unchanged until trisolve_free.  A CSC plan owns a device
+ * transpose of the mirror.                                                                  */
+typedef struct sprs_b200_trisolve sprs_b200_trisolve;
+enum { SPRS_B200_TRI_LOWER = 0, SPRS_B200_TRI_UPPER = 1 };
+/* the reason of a SingularMatrix, chosen from (storage, triangle) as the reference does:
+ * IS_ZERO "diagonal element is 0" (lsolve_csr), NUMERIC "diagonal element is a numeric 0"
+ * (usolve_csr; CSC forms with a stored 0), STRUCTURAL "diagonal element is a structural 0"
+ * (CSC forms without a stored diagonal)                                                      */
+enum {
+    SPRS_B200_SINGULAR_IS_ZERO = 0,
+    SPRS_B200_SINGULAR_NUMERIC = 1,
+    SPRS_B200_SINGULAR_STRUCTURAL = 2
+};
+/* ERR_DIMENSION if the matrix is not square, ERR_ARGUMENT for a bad triangle.  Blocking. */
+int sprs_b200_trisolve_plan(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, int tri,
+                            sprs_b200_trisolve** out);
+/* 1 and (index, reason) when a solve with this plan returns ERR_SINGULAR, else 0 */
+int sprs_b200_trisolve_singular(const sprs_b200_trisolve* plan, uint64_t* index, int* reason);
+/* rhs (host, len doubles) solved in place; blocking.  ERR_DIMENSION if len != n.  A singular
+ * plan returns ERR_SINGULAR after leaving rhs as the reference does: rows processed before the
+ * singular index solved, the others untouched (CSR) or holding b_r minus the terms of the
+ * columns processed before it (CSC).  Waits between rows are bounded by progress: ERR_CUDA
+ * (x incomplete) only if no row of the whole solve moved for ~9 s of GPU clock -- a bug report,
+ * never a valid input, however long a single wait lasts.  The plan stays usable after it.    */
+int sprs_b200_trisolve_solve(sprs_b200_trisolve* plan, double* rhs, uint64_t len);
+/* the same on a device vector of n doubles, enqueued on `stream` (asynchronous, like
+ * spmv_dev); returns ERR_SINGULAR (after enqueueing the same work) when the plan is singular.
+ * One stream at a time per plan.  A breach of the wait bound in a solve_dev is reported
+ * (ERR_CUDA, once) by the next solve or solve_dev of the plan, before it enqueues anything.  */
+int sprs_b200_trisolve_solve_dev(sprs_b200_trisolve* plan, double* d_rhs, void* stream);
+/* waits for the last solve enqueued with the plan (on its stream), then frees it */
+int sprs_b200_trisolve_free(sprs_b200_trisolve* plan);
 
 /* ---- measurement aid (bench.py roofline.gather_ceiling; not a product path): the SpMV's
  * memory behaviour on THIS matrix with the row logic removed -- the same (index, value) stream

@@ -621,6 +621,58 @@ class BiCGSTAB {
     sprs_b200_bicgstab* h_ = nullptr;
 };
 }  // namespace bicgstab
+
+// sprs::linalg::trisolve (linalg/trisolve.rs:30-262): L x = b / U x = b with a dense rhs solved
+// in place on the device, bit-identical to the reference.  The reference's panics throw Panic
+// in its order (square, then rhs.dim(), then storage); its Err(SingularMatrix) throws
+// SingularMatrix, with rhs left as the reference leaves it.
+struct SingularMatrix : std::runtime_error {  // LinalgError::SingularMatrix (errors.rs:59-69)
+    size_t index;
+    std::string reason;
+    SingularMatrix(size_t i, const std::string& r)
+        : std::runtime_error("Singular matrix at index " + std::to_string(i) + " (" + r + ")"),
+          index(i), reason(r) {}
+};
+namespace trisolve {
+namespace detail {
+template <class I, class Iptr>
+void solve(const CsMatI<I, Iptr>& mat, Array1& rhs, int tri, bool csr) {
+    if (mat.rows() != mat.cols()) throw Panic("Non square matrix passed to solver");
+    if (mat.cols() != rhs.size()) throw Panic("Dimension mismatch");
+    if (mat.is_csr() != csr) throw Panic("Storage mismatch");
+    Context& ctx = Context::thread_default();
+    sprs_b200_trisolve* plan = nullptr;
+    ctx.check(sprs_b200_trisolve_plan(ctx.handle(), mat.device(), tri, &plan));
+    const int st = sprs_b200_trisolve_solve(plan, rhs.data(), rhs.size());
+    uint64_t index = 0;
+    int reason = 0;
+    const bool singular = sprs_b200_trisolve_singular(plan, &index, &reason) != 0;
+    sprs_b200_trisolve_free(plan);
+    if (st == SPRS_B200_ERR_SINGULAR && singular) {
+        static const char* reasons[] = {"diagonal element is 0", "diagonal element is a numeric 0",
+                                        "diagonal element is a structural 0"};
+        throw SingularMatrix((size_t)index, reasons[reason]);
+    }
+    ctx.check(st);
+}
+}  // namespace detail
+template <class I, class Iptr>
+void lsolve_csr_dense_rhs(const CsMatI<I, Iptr>& lower_tri_mat, Array1& rhs) {
+    detail::solve(lower_tri_mat, rhs, SPRS_B200_TRI_LOWER, true);
+}
+template <class I, class Iptr>
+void usolve_csr_dense_rhs(const CsMatI<I, Iptr>& upper_tri_mat, Array1& rhs) {
+    detail::solve(upper_tri_mat, rhs, SPRS_B200_TRI_UPPER, true);
+}
+template <class I, class Iptr>
+void lsolve_csc_dense_rhs(const CsMatI<I, Iptr>& lower_tri_mat, Array1& rhs) {
+    detail::solve(lower_tri_mat, rhs, SPRS_B200_TRI_LOWER, false);
+}
+template <class I, class Iptr>
+void usolve_csc_dense_rhs(const CsMatI<I, Iptr>& upper_tri_mat, Array1& rhs) {
+    detail::solve(upper_tri_mat, rhs, SPRS_B200_TRI_UPPER, false);
+}
+}  // namespace trisolve
 }  // namespace linalg
 
 }  // namespace sprs

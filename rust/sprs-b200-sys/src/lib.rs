@@ -11,6 +11,7 @@ use std::os::raw::{c_char, c_double, c_int, c_void};
 #[repr(C)] pub struct sprs_b200_comm { _private: [u8; 0] }
 #[repr(C)] pub struct sprs_b200_symm { _private: [u8; 0] }
 #[repr(C)] pub struct sprs_b200_bicgstab { _private: [u8; 0] }
+#[repr(C)] pub struct sprs_b200_trisolve { _private: [u8; 0] }
 
 pub const SPRS_B200_CSR: c_int = 0;
 pub const SPRS_B200_CSC: c_int = 1;
@@ -26,6 +27,12 @@ pub const SPRS_B200_ERR_INDEX_RANGE: c_int = 5;
 pub const SPRS_B200_ERR_ARGUMENT: c_int = 6;
 pub const SPRS_B200_ERR_STRUCTURE: c_int = 7;
 pub const SPRS_B200_ERR_UNSUPPORTED: c_int = 8;
+pub const SPRS_B200_ERR_SINGULAR: c_int = 10;
+pub const SPRS_B200_TRI_LOWER: c_int = 0;
+pub const SPRS_B200_TRI_UPPER: c_int = 1;
+pub const SPRS_B200_SINGULAR_IS_ZERO: c_int = 0;
+pub const SPRS_B200_SINGULAR_NUMERIC: c_int = 1;
+pub const SPRS_B200_SINGULAR_STRUCTURAL: c_int = 2;
 pub const SPRS_B200_BICGSTAB_X: c_int = 0;
 pub const SPRS_B200_BICGSTAB_R: c_int = 1;
 pub const SPRS_B200_BICGSTAB_RHAT: c_int = 2;
@@ -104,6 +111,16 @@ extern "C" {
         x0: *const c_double, b: *const c_double, device_pointers: c_int,
         out: *mut *mut sprs_b200_bicgstab) -> c_int;
     pub fn sprs_b200_bicgstab_free(s: *mut sprs_b200_bicgstab) -> c_int;
+    // linalg::trisolve dense-rhs solves (trisolve.rs:30-262); the plan borrows the mirror
+    pub fn sprs_b200_trisolve_plan(
+        ctx: *mut sprs_b200_ctx, mat: *const sprs_b200_csmat, tri: c_int,
+        out: *mut *mut sprs_b200_trisolve) -> c_int;
+    pub fn sprs_b200_trisolve_singular(
+        plan: *const sprs_b200_trisolve, index: *mut u64, reason: *mut c_int) -> c_int;
+    pub fn sprs_b200_trisolve_solve(plan: *mut sprs_b200_trisolve, rhs: *mut c_double, len: u64) -> c_int;
+    pub fn sprs_b200_trisolve_solve_dev(
+        plan: *mut sprs_b200_trisolve, d_rhs: *mut c_double, stream: *mut c_void) -> c_int;
+    pub fn sprs_b200_trisolve_free(plan: *mut sprs_b200_trisolve) -> c_int;
     pub fn sprs_b200_bicgstab_step(s: *mut sprs_b200_bicgstab, err_out: *mut c_double) -> c_int;
     pub fn sprs_b200_bicgstab_soft_restart(s: *mut sprs_b200_bicgstab) -> c_int;
     pub fn sprs_b200_bicgstab_hard_restart(s: *mut sprs_b200_bicgstab) -> c_int;

@@ -312,3 +312,55 @@ pub mod bicgstab {
         pub fn p(&self) -> Array1<f64> { self.vec(ffi::SPRS_B200_BICGSTAB_P) }
     }
 }
+
+/// sprs::linalg::trisolve (linalg/trisolve.rs:30-262) on the device: `rhs` solved in place,
+/// bit-identical to the reference.  The reference's asserts panic with its messages in its
+/// order (square, `rhs.dim()`, storage); a singular matrix is
+/// `Err(LinalgError::SingularMatrix(SingularMatrixInfo { index, reason }))` with `rhs` left as
+/// the reference leaves it.
+pub mod linalg {
+    pub mod trisolve {
+        use super::super::*;
+        use sprs::errors::SingularMatrixInfo;
+
+        fn solve<I: SpIndex, Iptr: SpIndex>(mat: &DeviceCsMat<I, Iptr>, rhs: &mut [f64], tri: i32,
+                                            csr: bool) -> Result<(), LinalgError> {
+            assert_eq!(mat.host.cols(), mat.host.rows(), "Non square matrix passed to solver");
+            assert_eq!(mat.host.cols(), rhs.len(), "Dimension mismatch");
+            assert!(mat.host.is_csr() == csr, "Storage mismatch");
+            CTX.with(|c| {
+                let mut plan = std::ptr::null_mut();
+                check(c.0, unsafe { ffi::sprs_b200_trisolve_plan(c.0, mat.dev, tri, &mut plan) })?;
+                let st = unsafe { ffi::sprs_b200_trisolve_solve(plan, rhs.as_mut_ptr(), rhs.len() as u64) };
+                let (mut index, mut reason) = (0u64, 0i32);
+                let singular = unsafe { ffi::sprs_b200_trisolve_singular(plan, &mut index, &mut reason) } != 0;
+                unsafe { ffi::sprs_b200_trisolve_free(plan); }
+                if st == ffi::SPRS_B200_ERR_SINGULAR && singular {
+                    let reason = match reason {
+                        ffi::SPRS_B200_SINGULAR_IS_ZERO => "diagonal element is 0",
+                        ffi::SPRS_B200_SINGULAR_NUMERIC => "diagonal element is a numeric 0",
+                        _ => "diagonal element is a structural 0",
+                    };
+                    return Err(LinalgError::SingularMatrix(SingularMatrixInfo { index: index as usize, reason }));
+                }
+                check(c.0, st)
+            })
+        }
+        /// trisolve.rs:30-73
+        pub fn lsolve_csr_dense_rhs<I: SpIndex, Iptr: SpIndex>(lower_tri_mat: &DeviceCsMat<I, Iptr>, rhs: &mut [f64]) -> Result<(), LinalgError> {
+            solve(lower_tri_mat, rhs, ffi::SPRS_B200_TRI_LOWER, true)
+        }
+        /// trisolve.rs:219-262
+        pub fn usolve_csr_dense_rhs<I: SpIndex, Iptr: SpIndex>(upper_tri_mat: &DeviceCsMat<I, Iptr>, rhs: &mut [f64]) -> Result<(), LinalgError> {
+            solve(upper_tri_mat, rhs, ffi::SPRS_B200_TRI_UPPER, true)
+        }
+        /// trisolve.rs:85-149
+        pub fn lsolve_csc_dense_rhs<I: SpIndex, Iptr: SpIndex>(lower_tri_mat: &DeviceCsMat<I, Iptr>, rhs: &mut [f64]) -> Result<(), LinalgError> {
+            solve(lower_tri_mat, rhs, ffi::SPRS_B200_TRI_LOWER, false)
+        }
+        /// trisolve.rs:161-210
+        pub fn usolve_csc_dense_rhs<I: SpIndex, Iptr: SpIndex>(upper_tri_mat: &DeviceCsMat<I, Iptr>, rhs: &mut [f64]) -> Result<(), LinalgError> {
+            solve(upper_tri_mat, rhs, ffi::SPRS_B200_TRI_UPPER, false)
+        }
+    }
+}

@@ -6,10 +6,10 @@ Nothing here computes on the CPU: every product is a call into libsprs_b200.so
 creating a Context without one raises ThirdPartyError.
 """
 from . import _lib, io, linalg
-from .sparse import (CSC, CSR, Context, CsMat, CsVec, DeviceCsMat, SprsPanic, ThirdPartyError,
-                     binop, csmat_mul_csmat, prod, smmp)
+from .sparse import (CSC, CSR, Context, CsMat, CsVec, DeviceCsMat, SingularMatrix, SprsPanic,
+                     ThirdPartyError, binop, csmat_mul_csmat, prod, smmp)
 
-__all__ = ["CSC", "CSR", "Context", "CsMat", "CsVec", "DeviceCsMat", "SprsPanic",
+__all__ = ["CSC", "CSR", "Context", "CsMat", "CsVec", "DeviceCsMat", "SingularMatrix", "SprsPanic",
            "ThirdPartyError", "binop", "csmat_mul_csmat", "prod", "smmp", "_lib", "io", "linalg"]
 __version__ = "0.1.0"
 import os as _os

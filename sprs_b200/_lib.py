@@ -11,6 +11,9 @@ OK, ERR_DIMENSION, ERR_STORAGE, ERR_CUDA, ERR_NCCL, ERR_INDEX_RANGE, ERR_ARGUMEN
     ERR_STRUCTURE, ERR_UNSUPPORTED = range(9)
 CSR, CSC = 0, 1
 BINOP_ADD, BINOP_SUB, BINOP_MUL = 0, 1, 2
+ERR_SINGULAR = 10
+TRI_LOWER, TRI_UPPER = 0, 1
+SINGULAR_IS_ZERO, SINGULAR_NUMERIC, SINGULAR_STRUCTURAL = 0, 1, 2
 
 _vp, _u64, _i64, _int, _dp = C.c_void_p, C.c_uint64, C.c_int64, C.c_int, C.c_void_p
 _dense_sig = [_vp, _vp, _dp, _u64, _u64, _i64, _i64, _dp, _u64, _u64, _i64, _i64]
@@ -105,6 +108,11 @@ PROTOTYPES = {
     "sprs_b200_bicgstab_stats": (_int, [_vp, C.POINTER(_u64), C.POINTER(C.c_double)]),
     "sprs_b200_bicgstab_get": (_int, [_vp, _int, _dp, _u64]),
     "sprs_b200_bicgstab_get_dev": (_int, [_vp, _int, C.POINTER(_vp)]),
+    "sprs_b200_trisolve_plan": (_int, [_vp, _vp, _int, C.POINTER(_vp)]),
+    "sprs_b200_trisolve_singular": (_int, [_vp, C.POINTER(_u64), C.POINTER(_int)]),
+    "sprs_b200_trisolve_solve": (_int, [_vp, _dp, _u64]),
+    "sprs_b200_trisolve_solve_dev": (_int, [_vp, _dp, _vp]),
+    "sprs_b200_trisolve_free": (_int, [_vp]),
     "sprs_b200_diag_gather_ceiling": (_int, [_vp, _vp, _dp, _int, C.POINTER(C.c_double),
                                              C.POINTER(_u64)]),
     "sprs_b200_gen_rmat_keys": (_int, [_vp, _u64, _int, _u64, _u64, C.c_double, C.c_double,
@@ -118,7 +126,9 @@ PROTOTYPES = {
 _NOT_EMULATED = ("sprs_b200_comm_", "sprs_b200_symm_", "sprs_b200_partition_rows",
                  "sprs_b200_spmv_rowpart", "sprs_b200_mul_mat_vec_rowpart", "sprs_b200_diag_",
                  # the binops are in a separate emulated build (tests/emu_binop.py)
-                 "sprs_b200_csmat_binop", "sprs_b200_csmat_scale")
+                 "sprs_b200_csmat_binop", "sprs_b200_csmat_scale",
+                 # so are the triangular solves (tests/emu_trisolve.py)
+                 "sprs_b200_trisolve_")
 _lib = None
 
 

@@ -39,6 +39,17 @@ static __device__ __forceinline__ double ldg_stream_f64(const double* p, uint64_
     return v;
 }
 
+// ---- GPU-scope acquire / release on a u32 flag (the triangular solve's per-row ready flags):
+// the loads that follow an acquire see every store that preceded the matching release
+static __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
+    uint32_t v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+static __device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
 // ---- TMA bulk store shared -> global (bulk async-group completion); the destination may be a
 // peer GPU's memory or an NVSwitch multicast address
 static __device__ __forceinline__ void bulk_s2g(void* dst, const void* src_smem, uint32_t bytes) {

@@ -177,6 +177,58 @@ def make_matrix(ctx, gen, n, nnz_per_row, seed):
     return rand_csr(ctx, n, n, nnz_per_row, seed=seed)
 
 
+def triangular(ctx, a, lower=True):
+    """The strict lower (or upper) triangle of a square DeviceCsr `a` (a rand_csr / rmat_csr
+    key set) plus a diagonal d_r = 1 + sum |off-diagonal of row r|, as a new DeviceCsr: the
+    inputs of the triangular solves (csrc/trisolve.cu).  The dominant diagonal keeps x bounded.
+    Each row's sum is the difference of two entries of one float64 prefix sum of |a_rc| over the
+    whole triangle (torch.cumsum), so d_r equals 1 + sum |row| only to within the prefix sum's
+    rounding -- far inside the dominance the solves need."""
+    n = a.rows
+    dev = a.indices.device
+    ip = a.indptr.to(torch.int64) & 0xFFFFFFFF  # int32 storage of u32 values
+    rows = torch.repeat_interleave(torch.arange(n, device=dev, dtype=torch.int32), ip[1:] - ip[:-1])
+    keep = a.indices < rows if lower else a.indices > rows  # n < 2^31: u32 values fit int32
+    kr = rows[keep]
+    del rows
+    kc, kv = a.indices[keep], a.data[keep]
+    del keep
+    m = kc.numel()
+    cnt = torch.bincount(kr, minlength=n)
+    kip = torch.zeros(n + 1, device=dev, dtype=torch.int64)
+    torch.cumsum(cnt, 0, out=kip[1:])
+    cs = torch.zeros(m + 1, device=dev, dtype=torch.float64)
+    torch.cumsum(kv.abs(), 0, out=cs[1:])
+    diag = 1.0 + (cs[kip[1:]] - cs[kip[:-1]])
+    del cs
+    nip = kip + torch.arange(n + 1, device=dev, dtype=torch.int64)  # one diagonal per row
+    rank = torch.arange(m, device=dev, dtype=torch.int64) - kip[kr.to(torch.int64)]
+    pos = nip[kr.to(torch.int64)] + rank + (0 if lower else 1)
+    del rank, kr
+    indices = torch.empty(m + n, device=dev, dtype=torch.int32)
+    data = torch.empty(m + n, device=dev, dtype=torch.float64)
+    indices[pos] = kc
+    data[pos] = kv
+    del pos, kc, kv
+    dpos = nip[1:] - 1 if lower else nip[:-1]
+    indices[dpos] = torch.arange(n, device=dev, dtype=torch.int32)
+    data[dpos] = diag
+    _sync()
+    return DeviceCsr(ctx, n, n, nip.to(torch.int32), indices, data)
+
+
+def trisolve_dev(ctx, plan, x):
+    """Enqueue plan's solve of the device vector x (torch, float64, in place) on torch's current
+    stream; returns the SingularMatrix it raised, or None."""
+    from .sparse import SingularMatrix
+    try:
+        s = _stream_ptr()
+        plan.solve_dev(x.data_ptr(), s.value if s else None)
+    except SingularMatrix as e:
+        return e
+    return None
+
+
 def normal_vector(ctx, n, seed=0x5EED1002):
     x = torch.empty(n, device=_device(ctx), dtype=torch.float64)
     ctx.check(ctx.lib.sprs_b200_gen_normal_from_keys(ctx.h, seed, None, n, _dptr(x),

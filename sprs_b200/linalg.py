@@ -5,7 +5,11 @@
 `soft_restart`, `hard_restart` and accessors.  All vectors stay in HBM between iterations
 (csrc/solver.cu); this module only holds the handle.
 
-Differences a caller can see, both forced by the host language:
+`trisolve` mirrors sprs::linalg::trisolve (sprs/src/sparse/linalg/trisolve.rs): the four
+dense-rhs solves, bit-identical to the reference (csrc/trisolve.cu), and `TriSolvePlan` for
+repeated solves of one matrix and the device-resident form.
+
+Differences a caller can see in BiCGSTAB, both forced by the host language:
   * vectors are dense float64 arrays (a CsVec argument is densified; the reference's CsVec
     arithmetic is dense arithmetic on the union pattern, binop.rs:442-470), accessors return
     numpy arrays;
@@ -16,7 +20,8 @@ import ctypes as C
 
 import numpy as np
 
-from .sparse import CsMat, CsVec, DeviceCsMat, SprsPanic
+from . import _lib
+from .sparse import CsMat, CsVec, DeviceCsMat, SingularMatrix, SprsPanic
 
 _X, _R, _RHAT, _P, _B = range(5)
 
@@ -215,4 +220,127 @@ class bicgstab:  # noqa: N801  (module path of the reference: sprs::linalg::bicg
     NotConverged = NotConverged
 
 
-__all__ = ["BiCGSTAB", "NotConverged", "bicgstab"]
+_REASONS = {_lib.SINGULAR_IS_ZERO: "diagonal element is 0",
+            _lib.SINGULAR_NUMERIC: "diagonal element is a numeric 0",
+            _lib.SINGULAR_STRUCTURAL: "diagonal element is a structural 0"}
+
+
+class TriSolvePlan:
+    """The analysis of one matrix and triangle for repeated solves (sprs_b200_trisolve_plan):
+    the diagonal of every row and the first singular index in processing order.  `mat` is a
+    CsMat or DeviceCsMat, square; lower=True solves L x = b, False U x = b, in the matrix's
+    storage (CSR: lsolve_csr / usolve_csr, CSC: lsolve_csc / usolve_csc).  The plan reads the
+    matrix's values when it is built: it must not change while the plan lives (a CsMat's device
+    mirror never does)."""
+
+    def __init__(self, mat, lower=True):
+        if isinstance(mat, CsMat):
+            rows, cols = mat.shape
+        elif isinstance(mat, DeviceCsMat):
+            rows, cols = mat.rows, mat.cols
+        else:
+            raise TypeError("mat must be a CsMat or a DeviceCsMat")
+        if rows != cols:
+            raise SprsPanic("Non square matrix passed to solver")
+        dev = mat.device() if isinstance(mat, CsMat) else mat
+        self._mat, self._dev, self._ctx, self.n = mat, dev, dev.ctx, rows
+        h = C.c_void_p()
+        st = self._ctx.lib.sprs_b200_trisolve_plan(
+            self._ctx.h, dev.h, _lib.TRI_LOWER if lower else _lib.TRI_UPPER, C.byref(h))
+        if st == _lib.ERR_DIMENSION:
+            raise SprsPanic("Non square matrix passed to solver")
+        self._ctx.check(st)
+        self._h = h
+
+    def singular(self):
+        """SingularMatrix every solve of this plan raises, or None."""
+        idx, reason = C.c_uint64(), C.c_int()
+        if not self._ctx.lib.sprs_b200_trisolve_singular(self._h, C.byref(idx), C.byref(reason)):
+            return None
+        return SingularMatrix(int(idx.value), _REASONS[reason.value])
+
+    def _status(self, st):
+        if st == _lib.ERR_SINGULAR:
+            raise self.singular()
+        self._ctx.check(st)
+
+    def solve(self, rhs):
+        """rhs (a contiguous float64 array of n entries) solved in place.  Raises SingularMatrix
+        after leaving rhs as the reference leaves it."""
+        _check_rhs(rhs)
+        if rhs.size != self.n:
+            raise SprsPanic("Dimension mismatch")
+        self._status(self._ctx.lib.sprs_b200_trisolve_solve(
+            self._h, rhs.ctypes.data_as(C.c_void_p), rhs.size))
+
+    def solve_dev(self, d_rhs, stream=None):
+        """Enqueue the solve of n doubles at device address d_rhs on `stream` (a cudaStream_t
+        as an int; None = the legacy default stream).  Asynchronous; raises SingularMatrix
+        (the work enqueued all the same) when the plan is singular.  One stream at a time."""
+        self._status(self._ctx.lib.sprs_b200_trisolve_solve_dev(
+            self._h, C.c_void_p(int(d_rhs)), C.c_void_p(int(stream) if stream else 0)))
+
+    def free(self):
+        if getattr(self, "_h", None):
+            self._ctx.lib.sprs_b200_trisolve_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def _check_rhs(rhs):
+    if not (isinstance(rhs, np.ndarray) and rhs.dtype == np.float64 and rhs.ndim == 1 and
+            rhs.flags.c_contiguous and rhs.flags.writeable):
+        raise TypeError("rhs must be a contiguous, writeable float64 array (DenseVectorMut)")
+
+
+def _dense_rhs_solve(mat, rhs, lower, csr):
+    """check_solver_dimensions (trisolve.rs:10-21), then the storage assert, then the solve."""
+    _check_rhs(rhs)
+    if not isinstance(mat, CsMat):
+        raise TypeError("mat must be a CsMat")
+    if mat.rows() != mat.cols():
+        raise SprsPanic("Non square matrix passed to solver")
+    if mat.cols() != rhs.size:
+        raise SprsPanic("Dimension mismatch")
+    if mat.is_csr() != csr:
+        raise SprsPanic("Storage mismatch")
+    plan = TriSolvePlan(mat, lower)
+    try:
+        plan.solve(rhs)
+    finally:
+        plan.free()
+
+
+class trisolve:  # noqa: N801  (module path of the reference: sprs::linalg::trisolve)
+    """Free functions of sprs/src/sparse/linalg/trisolve.rs.  `rhs` is solved in place; a
+    singular matrix raises SingularMatrix (the reference's Err(LinalgError::SingularMatrix))
+    with rhs left as the reference leaves it."""
+    TriSolvePlan = TriSolvePlan
+
+    @staticmethod
+    def lsolve_csr_dense_rhs(lower_tri_mat, rhs):
+        """trisolve.rs:30-73."""
+        _dense_rhs_solve(lower_tri_mat, rhs, True, True)
+
+    @staticmethod
+    def usolve_csr_dense_rhs(upper_tri_mat, rhs):
+        """trisolve.rs:219-262."""
+        _dense_rhs_solve(upper_tri_mat, rhs, False, True)
+
+    @staticmethod
+    def lsolve_csc_dense_rhs(lower_tri_mat, rhs):
+        """trisolve.rs:85-149."""
+        _dense_rhs_solve(lower_tri_mat, rhs, True, False)
+
+    @staticmethod
+    def usolve_csc_dense_rhs(upper_tri_mat, rhs):
+        """trisolve.rs:161-210."""
+        _dense_rhs_solve(upper_tri_mat, rhs, False, False)
+
+
+__all__ = ["BiCGSTAB", "NotConverged", "bicgstab", "TriSolvePlan", "trisolve"]

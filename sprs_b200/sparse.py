@@ -42,6 +42,16 @@ class ThirdPartyError(RuntimeError):
         self.msg = msg
 
 
+class SingularMatrix(ArithmeticError):
+    """LinalgError::SingularMatrix(SingularMatrixInfo{index, reason}) (sprs/src/errors.rs:59-69),
+    displayed as the reference displays it: "Singular matrix at index {index} ({reason})"."""
+
+    def __init__(self, index, reason):
+        super().__init__("Singular matrix at index %d (%s)" % (index, reason))
+        self.index = index
+        self.reason = reason
+
+
 def _ptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None and a.size else C.c_void_p(0)
 
@@ -78,6 +88,9 @@ class Context:
             raise SprsPanic("Storage mismatch")
         if st == _lib.ERR_INDEX_RANGE:
             raise SprsPanic(msg or "Index type is not large enough to hold the value")
+        if st == _lib.ERR_SINGULAR:  # message: "Singular matrix at index {i} ({reason})"
+            head, _, reason = msg.partition(" (")
+            raise SingularMatrix(int(head.rsplit(" ", 1)[-1]), reason[:-1])
         raise ThirdPartyError(st, msg)
 
     def synchronize(self):
