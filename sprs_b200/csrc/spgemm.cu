@@ -23,13 +23,17 @@
 //     <= 128   one warp per row, 256-slot hash map; A's non-zeros are applied ONE AT A
 //              TIME in storage order with the lanes across the B row, so every C value
 //              is the reference's sequential unfused sum -> bit-identical values;
-//     <= 4096  one CTA per row, up-to-8192-slot hash map in shared memory (96 KB),
-//              shared-memory f64 atomics, then an in-place bitonic sort by column;
-//     larger   one CTA per row, dense f64 accumulator over B.cols in a global-memory
-//              slot (the reference's `tmp`) + bitmap; extraction walks the bitmap in
-//              order, so the row comes out sorted, and re-zeroes what it touched.
-//   The two larger bins add in arrival order (f64 atomics): values agree with the
-//   reference to rounding (gate 1e-6 * sum|terms|), indices/indptr exactly.
+//     <= 1024  one CTA per row, hash map in shared memory (up to 2048 of its 8192 slots),
+//              then an in-place bitonic sort by column;
+//     larger   one CTA per row: <= 4096 A non-zeros, dense f64 accumulation in shared
+//              memory one 16384-column panel at a time; more ("hub" rows), a dense f64
+//              accumulator over B.cols in a global-memory slot (the reference's `tmp`) +
+//              bitmap; extraction walks the bitmap in order, so the row comes out sorted,
+//              and re-zeroes what it touched.
+//   The CTA-per-row bins add in the reference's order too, without f64 atomics: rounds of
+//   one A non-zero per warp, products staged in storage order and folded by one warp, long
+//   B rows finished by the whole CTA in turn (ordered_round) -> every value, index and
+//   indptr entry bit-identical to the reference, under any thread schedule.
 // Algorithmic bytes (SURVEY 8d): 12*(nnzA + n_prod + nnzC) + 8*(rows+1).
 
 #include <cstdlib>
@@ -65,9 +69,9 @@ constexpr uint64_t BITMAP_SMEM_MAX_COLS = 200ull * 1024 * 8;  // 200 KB of bits
 // serve only the rows they are cheap for -- with a shared-memory bitmap the symbolic phase sends
 // rows with n_prod > B.cols/256 to the bitmap kernel, the numeric phase rows with
 // nnz(C_i) > 16 * n_panels to the panel kernel; groups of G warps share one B row when the A row
-// is short (half of config 4's large rows have <= 8 A non-zeros); the CTA-per-row kernels run
-// 1024 threads and keep several 32-entry chunks of B in flight per warp: they are bound by the
-// L2 round trip of the B stream, not by the shared-memory atomics.
+// is short (half of config 4's large rows have <= 8 A non-zeros) in the symbolic kernels; the
+// symbolic bitmap kernel runs 1024 threads and keeps several 32-entry chunks of B in flight per
+// warp: it is bound by the L2 round trip of the B stream, not by the shared-memory atomics.
 
 // Warps that share one B row in the CTA-per-row kernels: the largest power of two G with
 // G * na <= nwarps (1 when grouping is off or the A row has at least nwarps/2 non-zeros).
@@ -339,6 +343,128 @@ __global__ void __launch_bounds__(NT)
     }
 }
 
+// ---- ordered accumulation for the CTA-per-row numeric kernels --------------------------
+// The reference adds a row's products into tmp[j] one A non-zero after the other, in storage
+// order, each sum starting from +0.0 (smmp.rs:173-181).  The CTA-per-row kernels keep that order
+// under any thread schedule without floating-point atomics: a CTA takes the row's A non-zeros in
+// rounds of one per warp, in storage order.  Each warp loads the first chunk (<= 32 products) of
+// its B-row segment and stages (slot, product) at its place in the round's stream, so the staged
+// list is in storage order; warp 0 then folds it into the accumulator.  A segment longer than one
+// chunk ("long") is finished by the whole CTA in turn, right after the staged products before it:
+// the products of one A non-zero have distinct columns, so its chunks need no order among
+// themselves.  `ACC_GLOBAL` bypasses L1 for an accumulator in global memory.
+template <bool ACC_GLOBAL>
+__device__ __forceinline__ double acc_load(const double* p) {
+    if constexpr (ACC_GLOBAL) return __ldcg(p);
+    else return *p;
+}
+template <bool ACC_GLOBAL>
+__device__ __forceinline__ void acc_store(double* p, double v) {
+    if constexpr (ACC_GLOBAL) __stcg(p, v);
+    else *p = v;
+}
+
+// warp 0: fold staged entries [s, e) into acc in stream order.  Lanes take 32 entries at a time;
+// equal slots are grouped with match_any and the group's lowest lane adds the members in lane
+// (= stream) order into the running value.
+template <bool ACC_GLOBAL, typename S>
+__device__ __forceinline__ void fold_staged(const S* st_slot, const double* st_val, uint32_t s,
+                                            uint32_t e, double* acc, int lane) {
+    for (uint32_t i = s; i < e; i += 32) {
+        const uint32_t j = i + lane;
+        const uint32_t slot = j < e ? (uint32_t)st_slot[j] : EMPTY;
+        const uint32_t grp = __match_any_sync(0xffffffffu, slot);
+        if (slot != EMPTY && (grp & ((1u << lane) - 1u)) == 0) {
+            double sum = acc_load<ACC_GLOBAL>(acc + slot);
+            for (uint32_t m = grp; m; m &= m - 1) sum = __dadd_rn(sum, st_val[i + __ffs(m) - 1]);
+            acc_store<ACC_GLOBAL>(acc + slot, sum);
+        }
+        __syncwarp();
+    }
+}
+
+// Per-round bookkeeping in shared memory for kernels whose segments are whole B rows (their
+// length is known up front): chunk counts, and for long segments the rest of the B row.
+struct RoundState {
+    uint32_t cnt[32];   // products staged by each warp
+    uint32_t rest0[32];  // long segments: first B position after the staged chunk
+    uint32_t rest1[32];  // long segments: end of the B row
+    double av[32];       // long segments: A's value
+};
+
+// One round of the ordered accumulation over whole B rows, A non-zeros [k0, k0 + nwarps).
+// `slot_of(col)` maps a column to its accumulator slot (order-free: a hash insert or the
+// column itself), `mark(col)` records the column for extraction.
+template <bool ACC_GLOBAL, typename SlotOf, typename Mark>
+__device__ __forceinline__ void ordered_round(
+    const uint32_t* __restrict__ a_idx, const double* __restrict__ a_val,
+    const uint32_t* __restrict__ b_ip, const uint32_t* __restrict__ b_idx,
+    const double* __restrict__ b_val, uint32_t k0, uint32_t a1, double* acc,
+    uint32_t* st_slot, double* st_val, RoundState& rs, SlotOf slot_of, Mark mark) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    const uint32_t k = k0 + warp;
+    uint32_t s = 0, len = 0;
+    double av = 0.0;
+    if (k < a1) {
+        const uint32_t br = a_idx[k];
+        s = b_ip[br];
+        len = b_ip[br + 1] - s;
+        av = a_val[k];
+    }
+    const uint32_t n = len < 32 ? len : 32;
+    uint32_t slot = EMPTY;
+    double prod = 0.0;
+    if ((uint32_t)lane < n) {
+        const uint32_t c = b_idx[s + lane];
+        prod = __dmul_rn(av, b_val[s + lane]);
+        slot = slot_of(c);
+        mark(c);
+    }
+    if (lane == 0) {
+        rs.cnt[warp] = n | (len > 32 ? 0x80000000u : 0u);
+        rs.rest0[warp] = s + 32;
+        rs.rest1[warp] = s + len;
+        rs.av[warp] = av;
+    }
+    __syncthreads();
+    // exclusive offsets of the warps' chunks in the round's stream (every warp computes them)
+    const uint32_t wc = lane < nwarps ? rs.cnt[lane] : 0u;
+    const uint32_t longs = __ballot_sync(0xffffffffu, wc >> 31);
+    uint32_t incl = wc & 0x7fffffffu;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += u;
+    }
+    const uint32_t off = __shfl_sync(0xffffffffu, incl, warp) - n;
+    const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+    if ((uint32_t)lane < n) {
+        st_slot[off + lane] = slot;
+        st_val[off + lane] = prod;
+    }
+    __syncthreads();
+    uint32_t from = 0;
+    for (uint32_t lm = longs; lm; lm &= lm - 1) {  // uniform
+        const int L = __ffs(lm) - 1;
+        const uint32_t upto = __shfl_sync(0xffffffffu, incl, L);
+        if (warp == 0) fold_staged<ACC_GLOBAL>(st_slot, st_val, from, upto, acc, lane);
+        __syncthreads();
+        const double lav = rs.av[L];
+        for (uint32_t p = rs.rest0[L] + threadIdx.x, e = rs.rest1[L]; p < e; p += blockDim.x) {
+            const uint32_t c = b_idx[p];
+            const uint32_t sl = slot_of(c);
+            mark(c);
+            acc_store<ACC_GLOBAL>(acc + sl, __dadd_rn(acc_load<ACC_GLOBAL>(acc + sl),
+                                                      __dmul_rn(lav, b_val[p])));
+        }
+        __syncthreads();
+        from = upto;
+    }
+    if (warp == 0) fold_staged<ACC_GLOBAL>(st_slot, st_val, from, total, acc, lane);
+    // the next round writes the stage only after its first barrier, which warp 0 reaches once
+    // its fold is done; `rs` is read above before the second barrier of this round
+}
+
 // ---- numeric, medium rows: CTA per row, hash map in shared memory + bitonic sort ----
 __global__ void __launch_bounds__(NT)
     num_med_kernel(const uint32_t* __restrict__ a_ip, const uint32_t* __restrict__ a_idx,
@@ -346,11 +472,13 @@ __global__ void __launch_bounds__(NT)
                    const uint32_t* __restrict__ b_idx, const double* __restrict__ b_val,
                    const uint64_t* __restrict__ c_ip, const uint32_t* __restrict__ cnt,
                    const uint32_t* __restrict__ list, uint32_t n_list,
-                   uint32_t* __restrict__ c_idx, double* __restrict__ c_val, int grouping) {
+                   uint32_t* __restrict__ c_idx, double* __restrict__ c_val) {
     extern __shared__ __align__(16) unsigned char dyn_raw[];
     double* tv = (double*)dyn_raw;                               // NUM_M_SLOTS doubles
     uint32_t* tk = (uint32_t*)(dyn_raw + NUM_M_SLOTS * sizeof(double));
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    __shared__ uint32_t st_slot[NT];
+    __shared__ double st_val[NT];
+    __shared__ RoundState rs;
     for (uint32_t li = blockIdx.x; li < n_list; li += gridDim.x) {
         const uint32_t r = list[li];
         const uint32_t n = cnt[r];
@@ -362,17 +490,14 @@ __global__ void __launch_bounds__(NT)
         }
         __syncthreads();
         const uint32_t a0 = a_ip[r], a1 = a_ip[r + 1];
-        const int G = warps_per_brow(a1 - a0, WARPS, grouping);
-        const int grp = warp / G, wg = warp % G, ngrp = WARPS / G;
-        for (uint32_t k = a0 + grp; k < a1; k += ngrp) {
-            const uint32_t br = a_idx[k];
-            const double av = a_val[k];
-            for (uint32_t p = b_ip[br] + wg * 32 + lane, pe = b_ip[br + 1]; p < pe; p += 32 * G) {
-                bool fresh;
-                const uint32_t slot = table_insert(tk, slots - 1, b_idx[p], &fresh);
-                atomicAdd(&tv[slot], __dmul_rn(av, b_val[p]));
-            }
-        }
+        auto slot_of = [&](uint32_t c) {
+            bool fresh;
+            return table_insert(tk, slots - 1, c, &fresh);
+        };
+        auto mark = [](uint32_t) {};
+        for (uint32_t k0 = a0; k0 < a1; k0 += WARPS)
+            ordered_round<false>(a_idx, a_val, b_ip, b_idx, b_val, k0, a1, tv, st_slot, st_val, rs,
+                                 slot_of, mark);
         __syncthreads();
         // in-place bitonic sort of (key, val) by key; EMPTY = +inf sinks to the end
         for (uint32_t size = 2; size <= slots; size <<= 1) {
@@ -418,22 +543,20 @@ __global__ void __launch_bounds__(1024)
     double* acc = g_acc + (uint64_t)blockIdx.x * cols;
     __shared__ uint32_t wsum[32];
     __shared__ uint32_t chunk_total;
+    __shared__ uint32_t st_slot[1024];
+    __shared__ double st_val[1024];
+    __shared__ RoundState rs;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t nt = blockDim.x, nwarps = blockDim.x >> 5;  // 256..1024 threads
     for (uint32_t li = blockIdx.x; li < n_list; li += gridDim.x) {
         const uint32_t r = list[li];
         for (uint32_t i = threadIdx.x; i < words; i += nt) bm[i] = 0;
         __syncthreads();
-        for (uint32_t k = a_ip[r] + warp, e = a_ip[r + 1]; k < e; k += nwarps) {
-            const uint32_t br = a_idx[k];
-            const double av = a_val[k];
-            for (uint32_t p = b_ip[br] + lane, pe = b_ip[br + 1]; p < pe; p += 32) {
-                const uint32_t c = b_idx[p];
-                atomicAdd(&acc[c], __dmul_rn(av, b_val[p]));
-                atomicOr(&bm[c >> 5], 1u << (c & 31));
-            }
-        }
-        __threadfence();
+        auto slot_of = [](uint32_t c) { return c; };
+        auto mark = [&](uint32_t c) { atomicOr(&bm[c >> 5], 1u << (c & 31)); };
+        for (uint32_t k0 = a_ip[r], a1 = a_ip[r + 1]; k0 < a1; k0 += nwarps)
+            ordered_round<true>(a_idx, a_val, b_ip, b_idx, b_val, k0, a1, acc, st_slot, st_val, rs,
+                                slot_of, mark);
         __syncthreads();
         // ordered extraction: walk the bitmap 256 words at a time
         uint64_t out = c_ip[r];
@@ -481,12 +604,14 @@ __global__ void __launch_bounds__(1024)
 // non-zero a cursor remembers how far its (sorted) B row has been consumed, so every B entry is
 // read once and lands in the panel that owns its column; panels are extracted in order, so the
 // row comes out sorted.  No global atomics (round 1's dense accumulators in global memory were
-// 77 % of the whole SpGEMM).  What bounds it is the L2 round trip of the B stream, so:
-//   * everything a segment needs -- cursor, end of the B row, A's value -- sits in shared memory
-//     (filled once per row): one dependent global load per chunk instead of three;
-//   * a warp works on TWO A non-zeros at a time, index and value chunks of both in flight;
-//   * 1024 threads (32 warps of latency hiding at one CTA per SM), rows handed out dynamically,
-//     panels nothing landed in are skipped.
+// 77 % of the whole SpGEMM).  Everything a segment needs -- cursor, end of the B row, A's value
+// -- sits in shared memory (filled once per row): one dependent global load per chunk instead of
+// three; 1024 threads, rows handed out dynamically, panels nothing landed in are skipped.  The
+// products are added in the reference's order (see ordered_round): the round's stage keeps
+// 16-bit panel columns, so it fits beside the 210 KB below without shrinking PANEL_W or
+// PANEL_MAX_A.  On config 4 nearly every product comes from a B row longer than one chunk,
+// and each such segment costs the CTA a turn (two barriers, one L2 round trip): this kernel
+// takes 2.3x the time of the former arrival-order version there (DESIGN.md §11).
 constexpr uint32_t PANEL_W = 16384;       // columns per panel: 128 KB of f64 accumulators
 constexpr uint32_t PANEL_MAX_A = 4096;    // per-A-non-zero state: 16 B each = 64 KB
 constexpr size_t PANEL_SMEM = (size_t)PANEL_W * 8 + PANEL_W / 8 + (size_t)PANEL_MAX_A * 20;
@@ -512,6 +637,12 @@ __global__ void __launch_bounds__(PANEL_NT)
     __shared__ uint32_t chunk_total;
     __shared__ uint32_t panel_mark;  // sequence number of the last panel something landed in
     __shared__ uint32_t next_li;
+    // the round's stage (16-bit panel columns keep it beside the 210 KB above) and, per warp,
+    // its chunk count (bit 31: long), its A non-zero and a long segment's rest, end and A value
+    __shared__ uint16_t st_slot[NTH];
+    __shared__ double st_val[NTH];
+    __shared__ uint32_t lcnt[NWARPS], lkk[NWARPS], lrest[NWARPS], lend[NWARPS];
+    __shared__ double lav[NWARPS];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (uint32_t i = threadIdx.x; i < PANEL_W; i += NTH) acc[i] = 0.0;   // stays zero between rows
     for (uint32_t i = threadIdx.x; i < PANEL_W / 32; i += NTH) bm[i] = 0;
@@ -533,90 +664,91 @@ __global__ void __launch_bounds__(PANEL_NT)
             nextcol[kk] = 0;
         }
         __syncthreads();
-        // G warps share one B row when the A row is short (G > 1 implies na <= NWARPS / 2, so
-        // every group then sees at most one A non-zero per panel)
-        const int G = warps_per_brow(na, NWARPS, 1);
-        const int grp = warp / G, wg = warp % G, ngrp = NWARPS / G;
         uint64_t out = c_ip[r];
         for (uint32_t p0 = 0; p0 < cols; p0 += PANEL_W) {
             const uint32_t p1 = (cols - p0 > PANEL_W) ? p0 + PANEL_W : cols;
             ++seq;
-            uint32_t grp_taken = 0;  // G > 1: entries of the group's B row this warp consumed
-            bool landed = false;
-            // two A non-zeros (kk, kk + ngrp) per pass, their chunks interleaved
-            for (uint32_t kk = grp; kk < na; kk += 2 * ngrp) {
-                const uint32_t kb = kk + ngrp;
-                const bool has_b = kb < na;
-                // (G == 1 only: the first column beyond the cursor is known from the last visit)
-                const bool skip_a = G == 1 && nextcol[kk] >= p1;
-                const bool skip_b = !has_b || (G == 1 && nextcol[kb] >= p1);
-                if (skip_a && skip_b) continue;
-                const uint32_t base_a = cursor[kk], end_a = bend[kk];
-                const uint32_t base_b = has_b ? cursor[kb] : 0u, end_b = has_b ? bend[kb] : 0u;
-                const double av_a = aval[kk], av_b = has_b ? aval[kb] : 0.0;
-                // columns ascend, so the entries below p1 are a prefix of [base, end): a chunk
-                // inside the prefix is taken whole, the chunk holding its end partly, later
-                // chunks not at all -- with G warps the warps' counts add up to the prefix length
-                uint32_t pos_a = base_a + (uint32_t)wg * 32, pos_b = base_b + (uint32_t)wg * 32;
-                uint32_t taken_a = 0, taken_b = 0;
-                uint32_t next_a = EMPTY, next_b = EMPTY;  // first column NOT taken (EMPTY: row used up)
-                bool live_a = !skip_a && pos_a < end_a, live_b = !skip_b && pos_b < end_b;
-                while (live_a || live_b) {
-                    uint32_t ca = EMPTY, cb = EMPTY;
-                    double va = 0.0, vb = 0.0;
-                    const uint32_t pa = pos_a + lane, pb = pos_b + lane;
-                    if (live_a && pa < end_a) {
-                        ca = b_idx[pa];
-                        va = b_val[pa];
+            // ordered accumulation (see ordered_round): rounds of one A non-zero per warp; the
+            // segment of A non-zero kk in this panel is the prefix of [cursor, end) below p1
+            // (columns ascend), its first chunk is staged, a longer one is finished by the CTA
+            for (uint32_t k0 = 0; k0 < na; k0 += NWARPS) {
+                // (the first column beyond the cursor is known from the last visit, 0 = unknown)
+                const uint32_t kk = k0 + warp < na && nextcol[k0 + warp] < p1 ? k0 + warp : EMPTY;
+                uint32_t n = 0, pos = 0, end = 0, c = EMPTY;
+                bool lng = false;
+                double av = 0.0, v = 0.0;
+                uint32_t nxt = 0;
+                if (kk != EMPTY) {
+                    pos = cursor[kk];
+                    end = bend[kk];
+                    av = aval[kk];
+                    if (pos + lane < end) {
+                        c = b_idx[pos + lane];
+                        v = b_val[pos + lane];
                     }
-                    if (live_b && pb < end_b) {
-                        cb = b_idx[pb];
-                        vb = b_val[pb];
-                    }
-                    if (live_a) {
-                        const bool take = ca < p1;
-                        if (take) {
-                            atomicAdd(&acc[ca - p0], __dmul_rn(av_a, va));
-                            atomicOr(&bm[(ca - p0) >> 5], 1u << ((ca - p0) & 31));
-                        }
-                        const uint32_t n = __popc(__ballot_sync(0xffffffffu, take));
-                        taken_a += n;
-                        pos_a += 32u * G;
-                        live_a = n == 32 && pos_a < end_a;
-                        if (n < 32) next_a = __shfl_sync(0xffffffffu, ca, n);
-                    }
-                    if (live_b) {
-                        const bool take = cb < p1;
-                        if (take) {
-                            atomicAdd(&acc[cb - p0], __dmul_rn(av_b, vb));
-                            atomicOr(&bm[(cb - p0) >> 5], 1u << ((cb - p0) & 31));
-                        }
-                        const uint32_t n = __popc(__ballot_sync(0xffffffffu, take));
-                        taken_b += n;
-                        pos_b += 32u * G;
-                        live_b = n == 32 && pos_b < end_b;
-                        if (n < 32) next_b = __shfl_sync(0xffffffffu, cb, n);
-                    }
+                    n = __popc(__ballot_sync(0xffffffffu, c < p1));
+                    lng = n == 32 && pos + 32 < end;
+                    const uint32_t nc = __shfl_sync(0xffffffffu, c, n & 31);
+                    nxt = lng ? 0u : (n < 32 ? nc : EMPTY);  // EMPTY: row used up
+                    if (lane == 0 && n) panel_mark = seq;     // same value from every writer
                 }
-                landed |= (taken_a | taken_b) != 0;
-                if (G == 1) {
-                    if (lane == 0) {
-                        if (!skip_a) {
-                            cursor[kk] = base_a + taken_a;
-                            nextcol[kk] = next_a;  // (a chunk that ended exactly at `end`: EMPTY)
-                        }
-                        if (!skip_b) {
-                            cursor[kb] = base_b + taken_b;
-                            nextcol[kb] = next_b;
-                        }
-                    }
-                } else {
-                    grp_taken = taken_a;  // added after the barrier: the group's other warps read `base`
+                if (lane == 0) {
+                    lcnt[warp] = n | (lng ? 0x80000000u : 0u);
+                    lkk[warp] = kk;
+                    lrest[warp] = pos + 32;
+                    lend[warp] = end;
+                    lav[warp] = av;
                 }
+                __syncthreads();
+                if (kk != EMPTY && lane == 0) {
+                    cursor[kk] = pos + n;  // a long segment adds its rest below
+                    nextcol[kk] = nxt;
+                }
+                const uint32_t wc = lane < NWARPS ? lcnt[lane] : 0u;
+                const uint32_t longs = __ballot_sync(0xffffffffu, wc >> 31);
+                uint32_t incl = wc & 0x7fffffffu;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= o) incl += u;
+                }
+                const uint32_t off = __shfl_sync(0xffffffffu, incl, warp) - n;
+                const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+                if ((uint32_t)lane < n) {
+                    st_slot[off + lane] = (uint16_t)(c - p0);
+                    st_val[off + lane] = __dmul_rn(av, v);
+                    atomicOr(&bm[(c - p0) >> 5], 1u << ((c - p0) & 31));
+                }
+                __syncthreads();
+                uint32_t from = 0;
+                for (uint32_t lm = longs; lm; lm &= lm - 1) {  // uniform
+                    const int L = __ffs(lm) - 1;
+                    const uint32_t upto = __shfl_sync(0xffffffffu, incl, L);
+                    if (warp == 0) fold_staged<false>(st_slot, st_val, from, upto, acc, lane);
+                    __syncthreads();
+                    // the taken entries are a prefix: each warp stops at its first partial chunk
+                    const uint32_t q0 = lrest[L], e = lend[L];
+                    const double lv = lav[L];
+                    uint32_t mine = 0;
+                    for (uint32_t q = q0 + warp * 32u; q < e; q += NWARPS * 32u) {
+                        const uint32_t p = q + lane;
+                        const uint32_t cl = p < e ? b_idx[p] : EMPTY;
+                        const bool take = cl < p1;
+                        if (take) {
+                            acc[cl - p0] = __dadd_rn(acc[cl - p0], __dmul_rn(lv, b_val[p]));
+                            atomicOr(&bm[(cl - p0) >> 5], 1u << ((cl - p0) & 31));
+                        }
+                        const uint32_t nn = __popc(__ballot_sync(0xffffffffu, take));
+                        mine += nn;
+                        if (nn < 32) break;
+                    }
+                    if (lane == 0 && mine) atomicAdd(&cursor[lkk[L]], mine);
+                    __syncthreads();
+                    from = upto;
+                }
+                if (warp == 0) fold_staged<false>(st_slot, st_val, from, total, acc, lane);
             }
-            if (landed && lane == 0) panel_mark = seq;  // same value from every writer
             __syncthreads();
-            if (G > 1 && grp < (int)na && grp_taken && lane == 0) atomicAdd(&cursor[grp], grp_taken);
             if (panel_mark != seq) {  // nothing landed here (uniform: read after the barrier)
                 __syncthreads();      // cursor updates above / panel_mark before the next panel
                 continue;
@@ -767,7 +899,7 @@ int run_numeric(sprs_b200_ctx* ctx, sprs_b200_spgemm* p, uint32_t* d_cidx, doubl
         const unsigned g = std::min<unsigned>(h_cnt[1], cap);
         num_med_kernel<<<g, NT, smem, s>>>(a_ip, a->d_indices, a->d_data, b_ip, b->d_indices,
                                            b->d_data, p->d_cptr, p->d_cnt, l1, h_cnt[1], d_cidx,
-                                           d_cval, 1);
+                                           d_cval);
         ctx->launches += 1;
     }
     if (h_cnt[2]) {

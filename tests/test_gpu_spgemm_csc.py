@@ -1,11 +1,11 @@
 """GPU parity tests for SpGEMM (smmp.rs) and the CSC side of the dispatch tables
-(csmat.rs:1895-1949, 2009-2046), through the C ABI.  SpGEMM indptr / indices must be
-bit-exact; values within 1e-6 * sum|terms| (BASELINE north_star) and bit-exact where the
-kernel applies A's non-zeros in storage order (rows with nnz(C_i) <= 128)."""
+(csmat.rs:1895-1949, 2009-2046), through the C ABI.  SpGEMM indptr / indices and every value
+must be bit-exact: every numeric bin adds A's non-zeros in storage order, like the reference."""
 import numpy as np
 import pytest
 import scipy.sparse as sp_
 
+import exact
 from conftest import mat_arrays, rand_csr
 
 pytestmark = pytest.mark.gpu
@@ -155,20 +155,14 @@ def test_sparse_dot_dense_all_storages(sp, fixtures):
 
 
 # ------------------------------------------------------------------ oracle parity, random
-def check_spgemm(sp, O, a, b, shape_a, shape_b, bit_exact_small=True):
+def check_spgemm(sp, O, a, b, shape_a, shape_b):
     A = sp.CsMat.new(shape_a, *a)
     B = sp.CsMat.new(shape_b, *b)
     C = A * B
     rip, rind, rd = O.mul_csr_csr(shape_a, a, shape_b, b, threads=1)
     assert np.array_equal(C.indptr, rip), "indptr differs"
     assert np.array_equal(C.indices, rind), "indices differ"
-    absC = O.mul_csr_csr(shape_a, (a[0], a[1], np.abs(a[2])), shape_b,
-                         (b[0], b[1], np.abs(b[2])), threads=1)[2]
-    assert np.all(np.abs(C.data - rd) <= RTOL * absC + 1e-300)
-    if bit_exact_small:
-        lens = np.diff(rip.astype(np.int64))
-        small = np.repeat(lens <= 128, lens)
-        assert np.array_equal(C.data[small], rd[small]), "small rows must be bit-exact"
+    exact.assert_same_class(C.data, rd, "spgemm values")
     return C
 
 

@@ -7,12 +7,12 @@ their switch to the whole warp above 16 G non-zeros, the 31-row blocks; the SpMM
 (64 / 128 columns per pass); the SpGEMM bins (128 / 1024 C entries, 4096 A non-zeros, 16384-column
 panels) -- are pushed through the C ABI of the emulated library and compared with the oracle:
 SpMV (values within the parity gate, bit-exact where the design promises it), SpMM (bit-exact),
-SpGEMM (indptr / indices bit-exact, values within the gate), CSR<->CSC (bit-exact), triplets
+SpGEMM (bit-exact, values too: every bin adds in the reference's order), CSR<->CSC (bit-exact), triplets
 (pattern bit-exact), CSR x sparse vector (bit-exact).
 
 Every odd seed runs in INTEGER mode (tests/exact.py): A, B, x and y0 are small integers, every
-sum is exact in f64 whatever its order, and the SpMV, SpGEMM and dense-product checks become
-bit-equality.
+sum is exact in f64 whatever its order, and the SpMV and dense-product checks become
+bit-equality.  SpGEMM values are compared bit for bit in both modes.
 
     python tools/fuzz_emu.py --seconds 300 [--seed 1] [--schedule random:3]
 
@@ -95,13 +95,14 @@ def make_csr(rng, rows, cols, lens, integer=False):
 
 
 def gate(got, ref, bound, what, bits=False):
-    """the parity gate; bits=True (integer mode: every sum exact) -> bit-equality instead"""
+    """the parity gate; bits=True -> bit-equality instead (NaN by class): integer mode, where
+    every sum is exact, and results summed in the reference's order"""
     if bits:
         g, r = np.ascontiguousarray(got, dtype=np.float64), np.ascontiguousarray(ref, dtype=np.float64)
-        bad = g.view(np.uint64) != r.view(np.uint64)
+        bad = (g.view(np.uint64) != r.view(np.uint64)) & ~(np.isnan(g) & np.isnan(r))
         if bad.any():
             i = int(np.flatnonzero(bad.ravel())[0])
-            return "%s: element %d got %r want %r (integer data: must be bit-exact)" % (
+            return "%s: element %d got %r want %r (must be bit-exact)" % (
                 what, i, g.flat[i], r.flat[i])
         return None
     bad = ~(np.abs(got - ref) <= 1e-6 * bound + 1e-300)
@@ -296,7 +297,7 @@ def one_case(sp, O, seed):
     else:
         _, _, cb = O.mul_csr_csr((rows, cols), (ip, ind, np.abs(finite)), (cols, bcols),
                                  (bip, bind, np.abs(bd)), threads=1)
-        e = gate(cm.data, cd, cb, "spgemm values", integer)
+        e = gate(cm.data, cd, cb, "spgemm values", True)
         if e:
             errs.append(e)
         # storage dispatch (csmat.rs:1895-1949): CSC operands route through transposes; the
@@ -311,7 +312,7 @@ def one_case(sp, O, seed):
                 g = got.to_other_storage() if want_csc else got
                 if not (np.array_equal(g.indptr, cip) and np.array_equal(g.indices, cind)):
                     errs.append("spgemm dispatch: pattern differs from CSR x CSR")
-                elif gate(g.data, cd, cb, "spgemm dispatch values", integer):
+                elif gate(g.data, cd, cb, "spgemm dispatch values", True):
                     errs.append("spgemm dispatch: values differ from CSR x CSR")
     # ---- row slices: slice_outer + proper_indptr upload (slicing.rs:65-89), SpMV on the view
     if rows >= 3:
