@@ -160,6 +160,12 @@ int sprs_b200_mul_mat_vec(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, const 
 int sprs_b200_csr_mul_csvec(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, uint64_t dim,
                             uint64_t v_nnz, const void* v_indices, int index_bytes,
                             const double* v_data, double* res, uint64_t res_len);
+/* The same dot products, each sum starting from res[i] instead of 0.0: res[i] is read, then
+ * overwritten.  CsVecBase::dot_dense (vec.rs:894-904) sums with `Iterator::sum`, whose f64
+ * fold starts from -0.0, so its mirrors pass res = {-0.0}.                               */
+int sprs_b200_csr_mul_csvec_acc(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, uint64_t dim,
+                                uint64_t v_nnz, const void* v_indices, int index_bytes,
+                                const double* v_data, double* res, uint64_t res_len);
 
 /* ---- sparse x dense matrix, HOST buffers; rhs/out are ndarray views, strides in
  * ELEMENTS (may be negative/any, like ArrayView).  out += lhs * rhs.

@@ -484,15 +484,16 @@ CsVecI<I> operator*(const CsMatI<I, Iptr>& a, const CsVecI<I>& v) {
 // Sum of v1[i] * rhs[i] over the common pattern in ascending index order (dot_acc,
 // vec.rs:846-881) on the device: row_view(v1) through the merge-dot kernel (csrc/csvec.cu),
 // the reference's terms in the reference's order.
+// Every term is added, one by one, to `start`.
 template <class I>
 double merge_dot(const CsVecI<I>& v1, size_t dim, const std::vector<I>& idx,
-                 const std::vector<double>& dat) {
-    if (v1.nnz() == 0 || idx.empty()) return 0.0;
+                 const std::vector<double>& dat, double start = 0.0) {
+    if (v1.nnz() == 0 || idx.empty()) return start;
     auto row = CsMatI<I, I>::new_({1, dim}, {(I)0, (I)v1.nnz()}, v1.indices, v1.data);
     Context& ctx = Context::thread_default();
-    double y = 0.0;
-    ctx.check(sprs_b200_csr_mul_csvec(ctx.handle(), row.device(), dim, idx.size(), idx.data(),
-                                      (int)sizeof(I), dat.data(), &y, 1));
+    double y = start;
+    ctx.check(sprs_b200_csr_mul_csvec_acc(ctx.handle(), row.device(), dim, idx.size(), idx.data(),
+                                          (int)sizeof(I), dat.data(), &y, 1));
     return y;
 }
 // CsVecBase::dot (vec.rs:825-881) with a sparse rhs; panics if the dimensions differ
@@ -501,13 +502,16 @@ double dot(const CsVecI<I>& v1, const CsVecI<I>& v2) {
     if (v1.dim != v2.dim) throw Panic("Dimension mismatch");
     return merge_dot(v1, v1.dim, v2.indices, v2.data);
 }
-// CsVecBase::dot_dense (vec.rs:894-904) / dot with a dense rhs
+// CsVecBase::dot_dense (vec.rs:894-904): `Iterator::sum` of the products, and std's f64 sum
+// folds from -0.0 (rust-lang/rust#129321), where dot with a dense rhs (dot_acc) starts from
+// +0.0.  An empty vector, or one whose every product is -0.0, gives -0.0.
 template <class I>
 double dot_dense(const CsVecI<I>& v1, const Array1& rhs) {
     if (v1.dim != rhs.size()) throw Panic("Dimension mismatch");
     std::vector<I> all(rhs.size());
     for (size_t i = 0; i < all.size(); ++i) all[i] = (I)i;
-    return merge_dot(v1, v1.dim, all, std::vector<double>(rhs.data(), rhs.data() + rhs.size()));
+    return merge_dot(v1, v1.dim, all, std::vector<double>(rhs.data(), rhs.data() + rhs.size()),
+                     -0.0);
 }
 namespace prod {
 // prod::csvec_dot_by_binary_search (prod.rs:13-72): the same sum (matching entries in

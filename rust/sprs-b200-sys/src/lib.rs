@@ -79,6 +79,10 @@ extern "C" {
         ctx: *mut sprs_b200_ctx, mat: *const sprs_b200_csmat, dim: u64, v_nnz: u64,
         v_indices: *const c_void, index_bytes: c_int, v_data: *const c_double,
         res: *mut c_double, res_len: u64) -> c_int;
+    pub fn sprs_b200_csr_mul_csvec_acc(
+        ctx: *mut sprs_b200_ctx, mat: *const sprs_b200_csmat, dim: u64, v_nnz: u64,
+        v_indices: *const c_void, index_bytes: c_int, v_data: *const c_double,
+        res: *mut c_double, res_len: u64) -> c_int;
     pub fn sprs_b200_csr_mulacc_dense_rowmaj(
         ctx: *mut sprs_b200_ctx, lhs: *const sprs_b200_csmat, rhs: *const c_double,
         rhs_rows: u64, rhs_cols: u64, rhs_rs: i64, rhs_cs: i64, out: *mut c_double,

@@ -54,6 +54,7 @@ PROTOTYPES = {
     "sprs_b200_mul_acc_mat_vec_csc": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
     "sprs_b200_mul_mat_vec": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
     "sprs_b200_csr_mul_csvec": (_int, [_vp, _vp, _u64, _u64, _vp, _int, _dp, _dp, _u64]),
+    "sprs_b200_csr_mul_csvec_acc": (_int, [_vp, _vp, _u64, _u64, _vp, _int, _dp, _dp, _u64]),
     "sprs_b200_csr_mulacc_dense_rowmaj": (_int, _dense_sig),
     "sprs_b200_csr_mulacc_dense_colmaj": (_int, _dense_sig),
     "sprs_b200_csc_mulacc_dense_rowmaj": (_int, _dense_sig),

@@ -36,14 +36,15 @@ __global__ void __launch_bounds__(CSVEC_NT)
     csr_mul_csvec_kernel(const P* __restrict__ indptr, const uint32_t* __restrict__ indices,
                          const double* __restrict__ data, const double* __restrict__ x,
                          const unsigned char* __restrict__ present, double* __restrict__ y,
-                         uint64_t rows) {
+                         uint64_t rows, int accumulate) {
     constexpr unsigned FULL = 0xffffffffu;
     const int lane = threadIdx.x & 31;
     const uint64_t warp0 = (blockIdx.x * (uint64_t)CSVEC_NT + threadIdx.x) >> 5;
     const uint64_t nwarps = ((uint64_t)gridDim.x * CSVEC_NT) >> 5;
     for (uint64_t row = warp0; row < rows; row += nwarps) {
         const uint64_t s = (uint64_t)indptr[row], e = (uint64_t)indptr[row + 1];
-        double acc = 0.0;  // N::zero(), identical in every lane
+        // N::zero(), or (accumulate) the caller's start value; identical in every lane
+        double acc = accumulate ? y[row] : 0.0;
         for (uint64_t k = s; k < e; k += 32) {
             bool hit = false;
             double prod = 0.0;
@@ -65,9 +66,9 @@ __global__ void __launch_bounds__(CSVEC_NT)
 
 }  // namespace
 
-int sprs_b200_csr_mul_csvec(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, uint64_t dim,
-                            uint64_t v_nnz, const void* v_indices, int index_bytes,
-                            const double* v_data, double* res, uint64_t res_len) {
+static int csr_mul_csvec(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, uint64_t dim,
+                         uint64_t v_nnz, const void* v_indices, int index_bytes,
+                         const double* v_data, double* res, uint64_t res_len, int accumulate) {
     if (!ctx || !mat) return SPRS_B200_ERR_ARGUMENT;
     // assert_eq!(lhs.cols(), rhs.dim(), "Dimension mismatch")  prod.rs:174
     if (mat->cols != dim || mat->rows != res_len)
@@ -101,6 +102,8 @@ int sprs_b200_csr_mul_csvec(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, uint
         SPRS_CUDA(ctx, cudaMemsetAsync(d_present, 0, dim, s));
         // x needs no clearing: entries without a presence mark are never read
     }
+    if (accumulate)
+        SPRS_CUDA(ctx, cudaMemcpyAsync(d_y, res, res_len * sizeof(double), cudaMemcpyHostToDevice, s));
     if (v_nnz) {
         SPRS_CUDA(ctx, cudaMemcpyAsync(d_vdata, v_data, v_nnz * 8, cudaMemcpyHostToDevice, s));
         SPRS_CUDA(ctx, cudaMemcpyAsync(d_vind, v_indices, v_nnz * (size_t)index_bytes,
@@ -120,14 +123,26 @@ int sprs_b200_csr_mul_csvec(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, uint
     if (mat->indptr_bytes == 4)
         csr_mul_csvec_kernel<uint32_t><<<(unsigned)blocks, CSVEC_NT, 0, s>>>(
             (const uint32_t*)mat->d_indptr, mat->d_indices, mat->d_data, (const double*)d_x,
-            (const unsigned char*)d_present, (double*)d_y, res_len);
+            (const unsigned char*)d_present, (double*)d_y, res_len, accumulate);
     else
         csr_mul_csvec_kernel<uint64_t><<<(unsigned)blocks, CSVEC_NT, 0, s>>>(
             (const uint64_t*)mat->d_indptr, mat->d_indices, mat->d_data, (const double*)d_x,
-            (const unsigned char*)d_present, (double*)d_y, res_len);
+            (const unsigned char*)d_present, (double*)d_y, res_len, accumulate);
     ctx->launches += 1;
     SPRS_CUDA(ctx, cudaGetLastError());
     SPRS_CUDA(ctx, cudaMemcpyAsync(res, d_y, res_len * sizeof(double), cudaMemcpyDeviceToHost, s));
     SPRS_CUDA(ctx, cudaStreamSynchronize(s));
     return SPRS_B200_OK;
+}
+
+int sprs_b200_csr_mul_csvec(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, uint64_t dim,
+                            uint64_t v_nnz, const void* v_indices, int index_bytes,
+                            const double* v_data, double* res, uint64_t res_len) {
+    return csr_mul_csvec(ctx, mat, dim, v_nnz, v_indices, index_bytes, v_data, res, res_len, 0);
+}
+
+int sprs_b200_csr_mul_csvec_acc(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, uint64_t dim,
+                                uint64_t v_nnz, const void* v_indices, int index_bytes,
+                                const double* v_data, double* res, uint64_t res_len) {
+    return csr_mul_csvec(ctx, mat, dim, v_nnz, v_indices, index_bytes, v_data, res, res_len, 1);
 }

@@ -200,19 +200,20 @@ class CsVec:
         return "CsVec(dim=%d, indices=%s, data=%s)" % (self.dim, self.indices.tolist(),
                                                         self.data.tolist())
 
-    def _merge_dot(self, dim, idx, dat):
+    def _merge_dot(self, dim, idx, dat, start=0.0):
         """Sum of self[i] * rhs[i] over the common pattern in ascending index order (dot_acc,
         vec.rs:846-881) on the device: row_view(self) through the merge-dot kernel
-        (csrc/csvec.cu) -- the reference's terms in the reference's order."""
+        (csrc/csvec.cu) -- the reference's terms in the reference's order, added one by one to
+        `start`."""
         if self.nnz() == 0 or len(idx) == 0:
-            return 0.0
+            return start
         row = CsMat((1, dim), np.array([0, self.nnz()]), self.indices, self.data)
         ctx = row.context()
         vi = np.ascontiguousarray(idx, dtype=np.uint64)
         vd = np.ascontiguousarray(dat, dtype=np.float64)
-        y = np.empty(1)
-        ctx.check(ctx.lib.sprs_b200_csr_mul_csvec(ctx.h, row.device().h, dim, vi.size, _ptr(vi), 8,
-                                                  _ptr(vd), _ptr(y), 1))
+        y = np.array([start], dtype=np.float64)
+        ctx.check(ctx.lib.sprs_b200_csr_mul_csvec_acc(ctx.h, row.device().h, dim, vi.size, _ptr(vi),
+                                                      8, _ptr(vd), _ptr(y), 1))
         return float(y[0])
 
     def dot(self, rhs):
@@ -223,14 +224,20 @@ class CsVec:
             if self.dim != rhs.dim:
                 raise SprsPanic("Dimension mismatch: %d != %d" % (self.dim, rhs.dim))
             return self._merge_dot(self.dim, rhs.indices, rhs.data)
-        return self.dot_dense(rhs)
-
-    def dot_dense(self, rhs):
-        """CsVecBase::dot_dense (vec.rs:894-904)."""
-        d = np.ascontiguousarray(rhs, dtype=np.float64)
+        d = np.ascontiguousarray(rhs, dtype=np.float64)  # dot_acc: the sum starts from +0.0
         if d.ndim != 1 or d.size != self.dim:
             raise SprsPanic("Dimension mismatch: %d != %d" % (self.dim, d.size))
         return self._merge_dot(self.dim, np.arange(self.dim, dtype=np.uint64), d)
+
+    def dot_dense(self, rhs):
+        """CsVecBase::dot_dense (vec.rs:894-904): `Iterator::sum` of the products, and std's
+        f64 sum folds from -0.0 (rust-lang/rust#129321), not from the +0.0 of dot_acc.  So an
+        empty vector, or one whose every product is -0.0, gives -0.0; any other result is the
+        same as dot_acc's.  (Pinned from the std source: no Rust toolchain runs these tests.)"""
+        d = np.ascontiguousarray(rhs, dtype=np.float64)
+        if d.ndim != 1 or d.size != self.dim:
+            raise SprsPanic("Dimension mismatch: %d != %d" % (self.dim, d.size))
+        return self._merge_dot(self.dim, np.arange(self.dim, dtype=np.uint64), d, start=-0.0)
 
     # `&v * &A` = row_view(v) * A (vec.rs:1084-1102)
     def __mul__(self, rhs):

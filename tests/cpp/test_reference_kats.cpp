@@ -124,6 +124,19 @@ static void csvec_products() {
     try { dot(v1, CsVec(9, {1, 3, 5, 7}, {2., 2., 2., 2.})); } catch (const Panic&) { p1 = true; }
     try { dot_dense(v1, Array1(9, 1.0)); } catch (const Panic&) { p2 = true; }
     CHECK(p1 && p2);
+    // dot_dense sums with `Iterator::sum`, whose f64 fold starts from -0.0 (std since
+    // rust-lang/rust#129321, inside the reference's rust-version 1.88; pinned from the std
+    // source, not from a run): an empty vector and all -0.0 products give -0.0.  dot with a
+    // dense rhs is dot_acc, which starts from +0.0.
+    Array1 zeros(8, 0.0);
+    CsVec empty8(8, {}, {}), neg(8, {1, 4, 6}, {-1., -2.5, -0.0});
+    CHECK(std::signbit(dot_dense(empty8, dense)) && dot_dense(empty8, dense) == 0.);
+    CHECK(std::signbit(dot_dense(neg, zeros)));                  // -1*0, -2.5*0, -0*0: all -0.0
+    CHECK(!std::signbit(dot_dense(v1, zeros)));                  // +0.0 products
+    CsVec mixed(8, {1, 4}, {-0.0, 2.});
+    CHECK(dot_dense(mixed, dense) == 10.);                       // -0.0 + 10
+    CHECK(!std::signbit(dot(neg, CsVec(8, {1, 4, 6}, {0., 0., 0.}))));  // dot_acc: +0.0 + -0.0
+    CHECK(!std::signbit(dot(empty8, v1)));
 }
 // prod.rs:503-595 dense products
 static void dense_products() {
