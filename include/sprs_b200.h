@@ -53,8 +53,9 @@ enum {
     SPRS_B200_ERR_STRUCTURE = 7,   /* indptr not monotone / index out of bounds          */
     SPRS_B200_ERR_UNSUPPORTED = 8,
     SPRS_B200_ERR_COMM = 9,        /* multi-GPU rendezvous / barrier failure; see last_error */
-    SPRS_B200_ERR_SINGULAR = 10    /* LinalgError::SingularMatrix (errors.rs:59-69); see
-                                      sprs_b200_trisolve_singular                           */
+    SPRS_B200_ERR_SINGULAR = 10,   /* LinalgError::SingularMatrix (errors.rs:59-69); see
+                                      sprs_b200_trisolve_singular, sprs_b200_ldl_singular   */
+    SPRS_B200_ERR_NOT_SYMMETRIC = 11 /* "Matrix is not symmetric" (sprs-ldl ldl_symbolic)   */
 };
 
 int sprs_b200_version(void);
@@ -442,6 +443,57 @@ int sprs_b200_trisolve_solve(sprs_b200_trisolve* plan, double* rhs, uint64_t len
 int sprs_b200_trisolve_solve_dev(sprs_b200_trisolve* plan, double* d_rhs, void* stream);
 /* waits for the last solve enqueued with the plan (on its stream), then frees it */
 int sprs_b200_trisolve_free(sprs_b200_trisolve* plan);
+
+/* ---- sparse LDL^T factorization L D L^T = P A P^T (the sprs-ldl crate, sprs-ldl/src/lib.rs:
+ * LdlSymbolic, LdlNumeric, ldl_symbolic, ldl_numeric, ldl_lsolve, ldl_ltsolve) and
+ * sprs::is_symmetric (sparse/symmetric.rs).  Bit-identical to the reference: L (CSC: colptr,
+ * row indices, values), D, x of solve and the first singular index.  Row k of P A P^T is the
+ * stored outer vector perm[k] of the matrix in its own storage, its indices j mapped to pinv[j]
+ * (a CSR or CSC mirror of a symmetric matrix gives the same factor).  The symbolic analysis
+ * runs on the host (the mirror's indptr and indices are downloaded once); the numeric
+ * factorization, its updates and the solves run on the device.  u32 index arrays: |L| >= 2^32
+ * is ERR_INDEX_RANGE.                                                                       */
+typedef struct sprs_b200_ldl sprs_b200_ldl;
+/* *out = 1 if mat is square and every entry has a transposed partner with an equal value
+ * (== : a NaN entry is not symmetric), else 0.  Blocking.                                    */
+int sprs_b200_is_symmetric(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, int* out);
+/* linalg::diag_solve (sparse/linalg.rs): x_i = x_i / diag_i, host arrays of len entries */
+int sprs_b200_diag_solve(sprs_b200_ctx* ctx, const double* diag, double* x, uint64_t len);
+/* LdlSymbolic::new_perm.  perm: host u32[n] (perm[k] = the outer vector that is row k), or NULL
+ * for the identity.  Checks in the reference's order: ERR_DIMENSION "matrix should be square",
+ * then (check_symmetry != 0) ERR_NOT_SYMMETRIC, then ERR_ARGUMENT for a perm that is not a
+ * permutation of 0..n-1.  Blocking; the mirror is not borrowed.                             */
+int sprs_b200_ldl_symbolic(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, const uint32_t* perm,
+                           int check_symmetry, sprs_b200_ldl** out);
+/* |L| (LdlSymbolic::nnz / LdlNumeric::nnz) of a symbolic or numeric handle */
+uint64_t sprs_b200_ldl_nnz(const sprs_b200_ldl* ldl);
+/* LdlSymbolic::factor: a numeric handle that BORROWS sym (sym must outlive it), factored from
+ * mat (same pattern as the symbolic's mat).  ERR_SINGULAR: *out is still set, holds no valid
+ * factor (solve, get_l and get_d return ERR_SINGULAR) and may be updated.  Blocking.        */
+int sprs_b200_ldl_factor(const sprs_b200_ldl* sym, const sprs_b200_csmat* mat,
+                         sprs_b200_ldl** out);
+/* LdlNumeric::update with new values.  mat's indptr and indices must equal the symbolic
+ * matrix's (the reference leaves another pattern unspecified): else ERR_STRUCTURE, nothing
+ * launched and the factor unchanged.  ERR_SINGULAR: no valid factor until an update succeeds
+ * (the reference keeps the partial factor readable).  Blocking.                               */
+int sprs_b200_ldl_update(sprs_b200_ldl* num, const sprs_b200_csmat* mat);
+/* 1 and the index when the last factor / update found D_k == 0 ("diagonal element is a numeric
+ * 0"; -0.0 counts, NaN does not; the first k in row order), else 0                           */
+int sprs_b200_ldl_singular(const sprs_b200_ldl* num, uint64_t* index);
+/* LdlNumeric::solve: x = A^-1 b for host arrays of len == n (b and x may be the same).
+ * Blocking.                                                                                  */
+int sprs_b200_ldl_solve(sprs_b200_ldl* num, const double* b, double* x, uint64_t len);
+/* the same for device arrays of n doubles, enqueued on `stream` (asynchronous; b and x may be
+ * the same).  One stream at a time per handle.                                                */
+int sprs_b200_ldl_solve_dev(sprs_b200_ldl* num, const double* d_b, double* d_x, void* stream);
+/* LdlNumeric::l / d: L in CSC (colptr n+1, indices and data nnz entries; any may be NULL) and
+ * D (len == n), host arrays.  Blocking.                                                        */
+int sprs_b200_ldl_get_l(const sprs_b200_ldl* num, uint32_t* colptr, uint32_t* indices,
+                        double* data);
+int sprs_b200_ldl_get_d(const sprs_b200_ldl* num, double* d, uint64_t len);
+/* frees a symbolic or numeric handle (free the numeric handles of a symbolic one first);
+ * waits for the last solve enqueued with it                                                   */
+int sprs_b200_ldl_free(sprs_b200_ldl* ldl);
 
 /* ---- measurement aid (bench.py roofline.gather_ceiling; not a product path): the SpMV's
  * memory behaviour on THIS matrix with the row logic removed -- the same (index, value) stream

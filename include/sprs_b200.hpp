@@ -677,6 +677,171 @@ void usolve_csc_dense_rhs(const CsMatI<I, Iptr>& upper_tri_mat, Array1& rhs) {
     detail::solve(upper_tri_mat, rhs, SPRS_B200_TRI_UPPER, false);
 }
 }  // namespace trisolve
+
+// sprs::linalg::diag_solve (sparse/linalg.rs): x_i /= diag_i on the device
+inline void diag_solve(const Array1& diag, Array1& x) {
+    if (diag.size() != x.size()) throw Panic("assertion `left == right` failed");
+    Context& ctx = Context::thread_default();
+    ctx.check(sprs_b200_diag_solve(ctx.handle(), diag.data(), x.data(), x.size()));
+}
 }  // namespace linalg
+
+// The sprs-ldl crate (sprs-ldl/src/lib.rs): L D L^T = P A P^T on the device with the permutation
+// given (new_perm) or the identity (new_), bit-identical L, D, x and singular index.  No
+// fill-reducing ordering is computed.  The reference's panics throw Panic in its order (square,
+// symmetry, permutation); Err(SingularMatrix) throws SingularMatrix.  After an update that
+// throws SingularMatrix, l, d and solve throw it too until an update succeeds; an update with
+// another pattern throws Panic before any work is done and leaves the factor as it was.
+namespace ldl {
+using linalg::SingularMatrix;
+enum class SymmetryCheck { CheckSymmetry, DontCheckSymmetry };
+namespace detail {
+static const char* const kNumericZero = "diagonal element is a numeric 0";
+struct Handle {
+    sprs_b200_ldl* h = nullptr;
+    explicit Handle(sprs_b200_ldl* p) : h(p) {}
+    Handle(const Handle&) = delete;
+    Handle& operator=(const Handle&) = delete;
+    ~Handle() { sprs_b200_ldl_free(h); }
+};
+inline void status(Context& ctx, int st, uint64_t index) {
+    if (st == SPRS_B200_ERR_NOT_SYMMETRIC) throw Panic("Matrix is not symmetric");
+    if (st == SPRS_B200_ERR_SINGULAR) throw SingularMatrix((size_t)index, kNumericZero);
+    if (st == SPRS_B200_ERR_STRUCTURE) throw Panic(sprs_b200_last_error(ctx.handle()));
+    ctx.check(st);
+}
+}  // namespace detail
+
+// sprs::is_symmetric (sparse/symmetric.rs) on the device
+template <class I, class Iptr>
+bool is_symmetric(const CsMatI<I, Iptr>& mat) {
+    Context& ctx = Context::thread_default();
+    int out = 0;
+    ctx.check(sprs_b200_is_symmetric(ctx.handle(), mat.device(), &out));
+    return out != 0;
+}
+
+class LdlNumeric;
+class LdlSymbolic {
+   public:
+    template <class I, class Iptr>
+    static LdlSymbolic new_(const CsMatI<I, Iptr>& mat) {
+        if (mat.rows() != mat.cols()) throw Panic("assertion `left == right` failed");
+        return build(mat, nullptr, SymmetryCheck::CheckSymmetry);
+    }
+    // perm[k] is the outer vector of mat that is row k of P A P^T
+    template <class I, class Iptr>
+    static LdlSymbolic new_perm(const CsMatI<I, Iptr>& mat, const std::vector<size_t>& perm,
+                                SymmetryCheck check) {
+        return build(mat, &perm, check);
+    }
+    size_t problem_size() const { return n_; }
+    size_t nnz() const { return (size_t)sprs_b200_ldl_nnz(h_->h); }
+    template <class I, class Iptr>
+    LdlNumeric factor(const CsMatI<I, Iptr>& mat) const;
+
+   private:
+    template <class I, class Iptr>
+    static LdlSymbolic build(const CsMatI<I, Iptr>& mat, const std::vector<size_t>* perm,
+                             SymmetryCheck check) {
+        const size_t n = mat.rows();
+        if (mat.cols() != n) throw Panic("matrix should be square");
+        const bool check_sym = check == SymmetryCheck::CheckSymmetry;
+        std::vector<uint32_t> p;
+        if (perm) {
+            if (perm->size() != n) {
+                if (check_sym && !is_symmetric(mat)) throw Panic("Matrix is not symmetric");
+                throw Panic("assertion failed: perm_is_valid(&perm)");
+            }
+            for (size_t v : *perm) p.push_back(v >= n ? (uint32_t)n : (uint32_t)v);
+        }
+        Context& ctx = Context::thread_default();
+        sprs_b200_ldl* h = nullptr;
+        const int st = sprs_b200_ldl_symbolic(ctx.handle(), mat.device(), perm ? p.data() : nullptr,
+                                              check_sym ? 1 : 0, &h);
+        if (st == SPRS_B200_ERR_ARGUMENT) throw Panic("assertion failed: perm_is_valid(&perm)");
+        if (st == SPRS_B200_ERR_DIMENSION) throw Panic("matrix should be square");
+        detail::status(ctx, st, 0);
+        LdlSymbolic s;
+        s.h_ = std::make_shared<detail::Handle>(h);
+        s.n_ = n;
+        return s;
+    }
+    std::shared_ptr<detail::Handle> h_;
+    size_t n_ = 0;
+    friend class LdlNumeric;
+};
+
+class LdlNumeric {
+   public:
+    template <class I, class Iptr>
+    static LdlNumeric new_(const CsMatI<I, Iptr>& mat) {
+        return LdlSymbolic::new_(mat).factor(mat);
+    }
+    template <class I, class Iptr>
+    static LdlNumeric new_perm(const CsMatI<I, Iptr>& mat, const std::vector<size_t>& perm,
+                               SymmetryCheck check) {
+        return LdlSymbolic::new_perm(mat, perm, check).factor(mat);
+    }
+    template <class I, class Iptr>
+    void update(const CsMatI<I, Iptr>& mat) {
+        Context& ctx = Context::thread_default();
+        const int st = sprs_b200_ldl_update(h_->h, mat.device());
+        uint64_t index = 0;
+        sprs_b200_ldl_singular(h_->h, &index);
+        detail::status(ctx, st, index);
+    }
+    Array1 solve(const Array1& rhs) const {
+        if (rhs.size() != sym_.n_) throw Panic("assertion `left == right` failed");
+        Context& ctx = Context::thread_default();
+        Array1 x(rhs.size());
+        status(ctx, sprs_b200_ldl_solve(h_->h, rhs.data(), x.data(), x.size()));
+        return x;
+    }
+    // L in CSC, its unit diagonal not stored
+    CsMatI<size_t> l() const {
+        Context& ctx = Context::thread_default();
+        const size_t n = sym_.n_, nnz = this->nnz();
+        std::vector<uint32_t> ip(n + 1), ind(nnz);
+        std::vector<double> data(nnz);
+        status(ctx, sprs_b200_ldl_get_l(h_->h, ip.data(), ind.data(), data.data()));
+        return CsMatI<size_t>::new_csc({n, n}, std::vector<size_t>(ip.begin(), ip.end()),
+                                       std::vector<size_t>(ind.begin(), ind.end()), std::move(data));
+    }
+    Array1 d() const {
+        Context& ctx = Context::thread_default();
+        Array1 out(sym_.n_);
+        status(ctx, sprs_b200_ldl_get_d(h_->h, out.data(), out.size()));
+        return out;
+    }
+    size_t problem_size() const { return sym_.n_; }
+    size_t nnz() const { return sym_.nnz(); }
+
+   private:
+    void status(Context& ctx, int st) const {
+        uint64_t index = 0;
+        sprs_b200_ldl_singular(h_->h, &index);
+        detail::status(ctx, st, index);
+    }
+    LdlSymbolic sym_;                     // the numeric handle borrows it: destroyed after h_
+    std::shared_ptr<detail::Handle> h_;
+    friend class LdlSymbolic;
+};
+
+template <class I, class Iptr>
+LdlNumeric LdlSymbolic::factor(const CsMatI<I, Iptr>& mat) const {
+    if (n_ <= 1) throw Panic("assertion failed: n > 1");  // DStack::with_capacity(n)
+    Context& ctx = Context::thread_default();
+    sprs_b200_ldl* h = nullptr;
+    const int st = sprs_b200_ldl_factor(h_->h, mat.device(), &h);
+    LdlNumeric num;
+    num.sym_ = *this;
+    if (h) num.h_ = std::make_shared<detail::Handle>(h);
+    uint64_t index = 0;
+    if (h) sprs_b200_ldl_singular(h, &index);
+    detail::status(ctx, st, index);
+    return num;
+}
+}  // namespace ldl
 
 }  // namespace sprs

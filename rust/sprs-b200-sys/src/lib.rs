@@ -12,6 +12,7 @@ use std::os::raw::{c_char, c_double, c_int, c_void};
 #[repr(C)] pub struct sprs_b200_symm { _private: [u8; 0] }
 #[repr(C)] pub struct sprs_b200_bicgstab { _private: [u8; 0] }
 #[repr(C)] pub struct sprs_b200_trisolve { _private: [u8; 0] }
+#[repr(C)] pub struct sprs_b200_ldl { _private: [u8; 0] }
 
 pub const SPRS_B200_CSR: c_int = 0;
 pub const SPRS_B200_CSC: c_int = 1;
@@ -28,6 +29,7 @@ pub const SPRS_B200_ERR_ARGUMENT: c_int = 6;
 pub const SPRS_B200_ERR_STRUCTURE: c_int = 7;
 pub const SPRS_B200_ERR_UNSUPPORTED: c_int = 8;
 pub const SPRS_B200_ERR_SINGULAR: c_int = 10;
+pub const SPRS_B200_ERR_NOT_SYMMETRIC: c_int = 11;
 pub const SPRS_B200_TRI_LOWER: c_int = 0;
 pub const SPRS_B200_TRI_UPPER: c_int = 1;
 pub const SPRS_B200_SINGULAR_IS_ZERO: c_int = 0;
@@ -125,6 +127,28 @@ extern "C" {
     pub fn sprs_b200_trisolve_solve_dev(
         plan: *mut sprs_b200_trisolve, d_rhs: *mut c_double, stream: *mut c_void) -> c_int;
     pub fn sprs_b200_trisolve_free(plan: *mut sprs_b200_trisolve) -> c_int;
+    // sprs-ldl LDL^T factorization and sprs::is_symmetric; a numeric handle borrows its
+    // symbolic one
+    pub fn sprs_b200_diag_solve(ctx: *mut sprs_b200_ctx, diag: *const c_double, x: *mut c_double,
+                                len: u64) -> c_int;
+    pub fn sprs_b200_is_symmetric(ctx: *mut sprs_b200_ctx, mat: *const sprs_b200_csmat,
+                                  out: *mut c_int) -> c_int;
+    pub fn sprs_b200_ldl_symbolic(ctx: *mut sprs_b200_ctx, mat: *const sprs_b200_csmat,
+                                  perm: *const u32, check_symmetry: c_int,
+                                  out: *mut *mut sprs_b200_ldl) -> c_int;
+    pub fn sprs_b200_ldl_nnz(ldl: *const sprs_b200_ldl) -> u64;
+    pub fn sprs_b200_ldl_factor(sym: *const sprs_b200_ldl, mat: *const sprs_b200_csmat,
+                                out: *mut *mut sprs_b200_ldl) -> c_int;
+    pub fn sprs_b200_ldl_update(num: *mut sprs_b200_ldl, mat: *const sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_ldl_singular(num: *const sprs_b200_ldl, index: *mut u64) -> c_int;
+    pub fn sprs_b200_ldl_solve(num: *mut sprs_b200_ldl, b: *const c_double, x: *mut c_double,
+                               len: u64) -> c_int;
+    pub fn sprs_b200_ldl_solve_dev(num: *mut sprs_b200_ldl, d_b: *const c_double,
+                                   d_x: *mut c_double, stream: *mut c_void) -> c_int;
+    pub fn sprs_b200_ldl_get_l(num: *const sprs_b200_ldl, colptr: *mut u32, indices: *mut u32,
+                               data: *mut c_double) -> c_int;
+    pub fn sprs_b200_ldl_get_d(num: *const sprs_b200_ldl, d: *mut c_double, len: u64) -> c_int;
+    pub fn sprs_b200_ldl_free(ldl: *mut sprs_b200_ldl) -> c_int;
     pub fn sprs_b200_bicgstab_step(s: *mut sprs_b200_bicgstab, err_out: *mut c_double) -> c_int;
     pub fn sprs_b200_bicgstab_soft_restart(s: *mut sprs_b200_bicgstab) -> c_int;
     pub fn sprs_b200_bicgstab_hard_restart(s: *mut sprs_b200_bicgstab) -> c_int;

@@ -364,3 +364,145 @@ pub mod linalg {
         }
     }
 }
+
+/// The sprs-ldl crate (sprs-ldl/src/lib.rs) on the device: `LdlSymbolic` / `LdlNumeric` with the
+/// reference's names, bit-identical L, D, x and singular index.  The permutation is the one
+/// given (`new_perm`) or the identity (`new`); no fill-reducing ordering is computed.  Panics
+/// follow the reference's order: square, symmetry (`CheckSymmetry`), permutation.  After an
+/// `update` that returns `Err(SingularMatrix)`, `l`, `d` and `solve` panic until an `update`
+/// succeeds; an `update` with another pattern panics before any work is done.
+pub mod ldl {
+    use super::*;
+    use sprs::errors::SingularMatrixInfo;
+    use sprs::SymmetryCheck;
+    use std::rc::Rc;
+
+    const NUMERIC_ZERO: &str = "diagonal element is a numeric 0";
+
+    struct Handle(*mut ffi::sprs_b200_ldl);
+    impl Drop for Handle { fn drop(&mut self) { unsafe { ffi::sprs_b200_ldl_free(self.0); } } }
+
+    fn status(ctx: *const ffi::sprs_b200_ctx, st: i32, index: u64) -> Result<(), LinalgError> {
+        match st {
+            ffi::SPRS_B200_ERR_NOT_SYMMETRIC => panic!("Matrix is not symmetric"),
+            ffi::SPRS_B200_ERR_SINGULAR => Err(LinalgError::SingularMatrix(SingularMatrixInfo {
+                index: index as usize, reason: NUMERIC_ZERO })),
+            ffi::SPRS_B200_ERR_STRUCTURE => panic!("{}", third_party(ctx, st)),
+            _ => check(ctx, st),
+        }
+    }
+
+    /// `sprs::is_symmetric` on the device.
+    pub fn is_symmetric<I: SpIndex, Iptr: SpIndex>(mat: &DeviceCsMat<I, Iptr>) -> bool {
+        CTX.with(|c| {
+            let mut out = 0;
+            check(c.0, unsafe { ffi::sprs_b200_is_symmetric(c.0, mat.dev, &mut out) }).unwrap();
+            out != 0
+        })
+    }
+
+    /// `sprs::linalg::diag_solve`: x_i /= diag_i on the device.
+    pub fn diag_solve(diag: &[f64], x: &mut [f64]) {
+        assert_eq!(diag.len(), x.len());
+        CTX.with(|c| check(c.0, unsafe {
+            ffi::sprs_b200_diag_solve(c.0, diag.as_ptr(), x.as_mut_ptr(), x.len() as u64) }).unwrap());
+    }
+
+    pub struct LdlSymbolic { h: Rc<Handle>, n: usize }
+    impl LdlSymbolic {
+        pub fn new<I: SpIndex, Iptr: SpIndex>(mat: &DeviceCsMat<I, Iptr>) -> Self {
+            assert_eq!(mat.host.rows(), mat.host.cols());
+            Self::new_perm(mat, None, SymmetryCheck::CheckSymmetry)
+        }
+        /// `perm[k]` is the outer vector of `mat` that is row k of P A P^T; `None`: identity.
+        pub fn new_perm<I: SpIndex, Iptr: SpIndex>(mat: &DeviceCsMat<I, Iptr>, perm: Option<&[usize]>,
+                                                  check_symmetry: SymmetryCheck) -> Self {
+            let n = mat.host.rows();
+            assert!(mat.host.cols() == n, "matrix should be square");
+            let p: Option<Vec<u32>> = perm.map(|p| p.iter().map(|&v| v.min(u32::MAX as usize) as u32).collect());
+            if let Some(p) = &p {
+                if p.len() != n {
+                    if check_symmetry == SymmetryCheck::CheckSymmetry && !is_symmetric(mat) {
+                        panic!("Matrix is not symmetric");
+                    }
+                    panic!("assertion failed: perm_is_valid(&perm)");
+                }
+            }
+            let check = (check_symmetry == SymmetryCheck::CheckSymmetry) as i32;
+            CTX.with(|c| {
+                let mut h = std::ptr::null_mut();
+                let pp = p.as_ref().map_or(std::ptr::null(), |p| p.as_ptr());
+                let st = unsafe { ffi::sprs_b200_ldl_symbolic(c.0, mat.dev, pp, check, &mut h) };
+                if st == ffi::SPRS_B200_ERR_ARGUMENT { panic!("assertion failed: perm_is_valid(&perm)"); }
+                if st == ffi::SPRS_B200_ERR_DIMENSION { panic!("matrix should be square"); }
+                status(c.0, st, 0).unwrap();
+                Self { h: Rc::new(Handle(h)), n }
+            })
+        }
+        pub fn problem_size(&self) -> usize { self.n }
+        pub fn nnz(&self) -> usize { unsafe { ffi::sprs_b200_ldl_nnz(self.h.0) as usize } }
+        pub fn factor<I: SpIndex, Iptr: SpIndex>(self, mat: &DeviceCsMat<I, Iptr>) -> Result<LdlNumeric, LinalgError> {
+            assert!(self.n > 1);  // DStack::with_capacity(n)
+            CTX.with(|c| {
+                let mut h = std::ptr::null_mut();
+                let st = unsafe { ffi::sprs_b200_ldl_factor(self.h.0, mat.dev, &mut h) };
+                let num = if h.is_null() { None } else { Some(Handle(h)) };
+                let mut index = 0u64;
+                if let Some(n) = &num { unsafe { ffi::sprs_b200_ldl_singular(n.0, &mut index); } }
+                status(c.0, st, index)?;
+                Ok(LdlNumeric { h: num.unwrap(), sym: self })
+            })
+        }
+    }
+
+    pub struct LdlNumeric { h: Handle, sym: LdlSymbolic }  // `h` drops before `sym`
+    impl LdlNumeric {
+        pub fn new<I: SpIndex, Iptr: SpIndex>(mat: &DeviceCsMat<I, Iptr>) -> Result<Self, LinalgError> {
+            LdlSymbolic::new(mat).factor(mat)
+        }
+        pub fn new_perm<I: SpIndex, Iptr: SpIndex>(mat: &DeviceCsMat<I, Iptr>, perm: &[usize],
+                                                  check_symmetry: SymmetryCheck) -> Result<Self, LinalgError> {
+            LdlSymbolic::new_perm(mat, Some(perm), check_symmetry).factor(mat)
+        }
+        pub fn update<I: SpIndex, Iptr: SpIndex>(&mut self, mat: &DeviceCsMat<I, Iptr>) -> Result<(), LinalgError> {
+            CTX.with(|c| {
+                let st = unsafe { ffi::sprs_b200_ldl_update(self.h.0, mat.dev) };
+                let mut index = 0u64;
+                unsafe { ffi::sprs_b200_ldl_singular(self.h.0, &mut index); }
+                status(c.0, st, index)
+            })
+        }
+        fn valid(&self) {
+            let mut index = 0u64;
+            if unsafe { ffi::sprs_b200_ldl_singular(self.h.0, &mut index) } != 0 {
+                panic!("Singular matrix at index {} ({})", index, NUMERIC_ZERO);
+            }
+        }
+        pub fn solve(&self, rhs: &[f64]) -> Vec<f64> {
+            assert_eq!(self.sym.n, rhs.len());
+            self.valid();
+            let mut x = vec![0.0; rhs.len()];
+            CTX.with(|c| check(c.0, unsafe {
+                ffi::sprs_b200_ldl_solve(self.h.0, rhs.as_ptr(), x.as_mut_ptr(), x.len() as u64) }).unwrap());
+            x
+        }
+        /// L in CSC, its unit diagonal not stored.
+        pub fn l(&self) -> CsMatI<f64, usize> {
+            self.valid();
+            let (n, nnz) = (self.sym.n, self.nnz());
+            let (mut ip, mut ind, mut data) = (vec![0u32; n + 1], vec![0u32; nnz], vec![0.0; nnz]);
+            CTX.with(|c| check(c.0, unsafe {
+                ffi::sprs_b200_ldl_get_l(self.h.0, ip.as_mut_ptr(), ind.as_mut_ptr(), data.as_mut_ptr()) }).unwrap());
+            CsMatI::new_csc((n, n), ip.into_iter().map(|v| v as usize).collect(),
+                            ind.into_iter().map(|v| v as usize).collect(), data)
+        }
+        pub fn d(&self) -> Vec<f64> {
+            self.valid();
+            let mut d = vec![0.0; self.sym.n];
+            CTX.with(|c| check(c.0, unsafe { ffi::sprs_b200_ldl_get_d(self.h.0, d.as_mut_ptr(), d.len() as u64) }).unwrap());
+            d
+        }
+        pub fn problem_size(&self) -> usize { self.sym.n }
+        pub fn nnz(&self) -> usize { self.sym.nnz() }
+    }
+}

@@ -5,12 +5,14 @@ Nothing here computes on the CPU: every product is a call into libsprs_b200.so
 (hand-written CUDA).  Importing works without a GPU (so the ABI can be inspected);
 creating a Context without one raises ThirdPartyError.
 """
-from . import _lib, io, linalg
+from . import _lib, io, ldl, linalg
+from .ldl import is_symmetric
 from .sparse import (CSC, CSR, Context, CsMat, CsVec, DeviceCsMat, SingularMatrix, SprsPanic,
                      ThirdPartyError, binop, csmat_mul_csmat, prod, smmp)
 
 __all__ = ["CSC", "CSR", "Context", "CsMat", "CsVec", "DeviceCsMat", "SingularMatrix", "SprsPanic",
-           "ThirdPartyError", "binop", "csmat_mul_csmat", "prod", "smmp", "_lib", "io", "linalg"]
+           "ThirdPartyError", "binop", "csmat_mul_csmat", "is_symmetric", "prod", "smmp", "_lib", "io",
+           "ldl", "linalg"]
 __version__ = "0.1.0"
 import os as _os
 

@@ -12,6 +12,7 @@ OK, ERR_DIMENSION, ERR_STORAGE, ERR_CUDA, ERR_NCCL, ERR_INDEX_RANGE, ERR_ARGUMEN
 CSR, CSC = 0, 1
 BINOP_ADD, BINOP_SUB, BINOP_MUL = 0, 1, 2
 ERR_SINGULAR = 10
+ERR_NOT_SYMMETRIC = 11
 TRI_LOWER, TRI_UPPER = 0, 1
 SINGULAR_IS_ZERO, SINGULAR_NUMERIC, SINGULAR_STRUCTURAL = 0, 1, 2
 
@@ -114,6 +115,18 @@ PROTOTYPES = {
     "sprs_b200_trisolve_solve": (_int, [_vp, _dp, _u64]),
     "sprs_b200_trisolve_solve_dev": (_int, [_vp, _dp, _vp]),
     "sprs_b200_trisolve_free": (_int, [_vp]),
+    "sprs_b200_diag_solve": (_int, [_vp, _dp, _dp, _u64]),
+    "sprs_b200_is_symmetric": (_int, [_vp, _vp, C.POINTER(_int)]),
+    "sprs_b200_ldl_symbolic": (_int, [_vp, _vp, _vp, _int, C.POINTER(_vp)]),
+    "sprs_b200_ldl_nnz": (_u64, [_vp]),
+    "sprs_b200_ldl_factor": (_int, [_vp, _vp, C.POINTER(_vp)]),
+    "sprs_b200_ldl_update": (_int, [_vp, _vp]),
+    "sprs_b200_ldl_singular": (_int, [_vp, C.POINTER(_u64)]),
+    "sprs_b200_ldl_solve": (_int, [_vp, _dp, _dp, _u64]),
+    "sprs_b200_ldl_solve_dev": (_int, [_vp, _dp, _dp, _vp]),
+    "sprs_b200_ldl_get_l": (_int, [_vp, _vp, _vp, _dp]),
+    "sprs_b200_ldl_get_d": (_int, [_vp, _dp, _u64]),
+    "sprs_b200_ldl_free": (_int, [_vp]),
     "sprs_b200_diag_gather_ceiling": (_int, [_vp, _vp, _dp, _int, C.POINTER(C.c_double),
                                              C.POINTER(_u64)]),
     "sprs_b200_gen_rmat_keys": (_int, [_vp, _u64, _int, _u64, _u64, C.c_double, C.c_double,
@@ -129,7 +142,9 @@ _NOT_EMULATED = ("sprs_b200_comm_", "sprs_b200_symm_", "sprs_b200_partition_rows
                  # the binops are in a separate emulated build (tests/emu_binop.py)
                  "sprs_b200_csmat_binop", "sprs_b200_csmat_scale",
                  # so are the triangular solves (tests/emu_trisolve.py)
-                 "sprs_b200_trisolve_")
+                 "sprs_b200_trisolve_",
+                 # and the LDL^T factorization (tests/emu_ldl.py)
+                 "sprs_b200_ldl_", "sprs_b200_is_symmetric", "sprs_b200_diag_solve")
 _lib = None
 
 

@@ -162,4 +162,53 @@ __device__ __forceinline__ uint64_t mix64(uint64_t z) {  // splitmix64 finaliser
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
     return z ^ (z >> 31);
 }
+
+// ---- progress-bounded waits on per-row ready flags (DESIGN.md 4.8), shared by the triangular
+// solves (trisolve.cu) and the LDL^T factorization (ldl.cu).  Rows are claimed by a ticket
+// counter in dependency order, so a wait always ends unless the whole launch stands still.
+// wait_ready is a template so that only the files that wait, and so include ptx.cuh, need the
+// definition of ld_acquire_u32.
+static __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p);  // ptx.cuh
+constexpr long long TRI_WAIT_BOUND = 1ll << 34;  // cycles: ~9 s at 1.98 GHz
+
+// The launch's progress: the sum of every warp's count (each only grows during a launch).
+__device__ __forceinline__ unsigned long long progress_sum(const unsigned long long* w, uint64_t n) {
+    unsigned long long sum = 0;
+    for (uint64_t i = 0; i < n; ++i) sum += __ldcg(w + i);
+    return sum;
+}
+
+// Wait until row c's flag holds `epoch`.  false: the launch's progress stood still for a whole
+// TRI_WAIT_BOUND interval (read only once a wait has lasted TRI_WAIT_BOUND: no cost before).
+template <typename Flag>
+__device__ __forceinline__ bool wait_ready(const Flag* flag, Flag epoch,
+                                           const unsigned long long* progress, uint64_t n_progress) {
+    if (ld_acquire_u32(flag) == epoch) return true;
+    long long start = clock64();
+    bool have = false;
+    unsigned long long seen = 0;
+    unsigned backoff = 32;
+    for (;;) {
+        __nanosleep(backoff);
+        if (ld_acquire_u32(flag) == epoch) return true;
+        if (backoff < 1024) backoff <<= 1;
+        if (clock64() - start > TRI_WAIT_BOUND) {
+            const unsigned long long now = progress_sum(progress, n_progress);
+            if (have && now == seen) return false;
+            have = true;  // the launch moved (or this is the first look): wait on
+            seen = now;
+            start = clock64();
+        }
+    }
+}
 #endif
+
+// ---- the triangular solve of trisolve.cu as a building block (ldl.cu): a plan for a
+// unit-diagonal triangle stored without its diagonal (no lookup, no division, never singular).
+// `csr` is borrowed and must outlive the plan; free it with sprs_b200_trisolve_free.
+int trisolve_unit_plan(sprs_b200_ctx* ctx, const sprs_b200_csmat* csr, int tri,
+                       sprs_b200_trisolve** out);
+// enqueue one solve of d_x in place on `s` (reports an earlier wait-bound breach first)
+int trisolve_enqueue(sprs_b200_trisolve* plan, double* d_x, cudaStream_t s);
+// ERR_CUDA once if a solve of the plan breached the wait bound, else OK
+int trisolve_check_breach(sprs_b200_trisolve* plan);

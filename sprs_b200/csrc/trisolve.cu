@@ -60,12 +60,12 @@ struct sprs_b200_trisolve {
     uint64_t k_ticket = 0;                 // first singular ticket (n: none)
     uint64_t sing_index = 0;
     int sing_reason = 0;
+    bool unit = false;                     // trisolve_unit_plan: no diagonal stored
 };
 
 namespace {
 
 constexpr int TRI_THREADS = 256;
-constexpr long long TRI_WAIT_BOUND = 1ll << 34;  // cycles: ~9 s at 1.98 GHz
 constexpr unsigned TRI_CTAS_PER_SM = 8;
 constexpr uint64_t TRI_HEARTBEAT = 32 * 256;      // terms of a long row between progress ticks
 
@@ -114,39 +114,10 @@ trisolve_plan_kernel(const P* __restrict__ ip, const uint32_t* __restrict__ idx,
         atomicMin(key, (unsigned long long)(ticket_of<UPPER>(r, n) << 1 | (present ? 1 : 0)));
 }
 
-// The solve's progress: the sum of every warp's count (each only grows during a launch).
-__device__ __forceinline__ unsigned long long progress_sum(const unsigned long long* w, uint64_t n) {
-    unsigned long long sum = 0;
-    for (uint64_t i = 0; i < n; ++i) sum += __ldcg(w + i);
-    return sum;
-}
-
-// Wait until row c's flag holds `epoch`.  false: the solve's progress stood still for a whole
-// TRI_WAIT_BOUND interval (read only once a wait has lasted TRI_WAIT_BOUND: no cost before).
-__device__ __forceinline__ bool wait_ready(const uint32_t* flag, uint32_t epoch,
-                                           const unsigned long long* progress, uint64_t n_progress) {
-    if (ld_acquire_u32(flag) == epoch) return true;
-    long long start = clock64();
-    bool have = false;
-    unsigned long long seen = 0;
-    unsigned backoff = 32;
-    for (;;) {
-        __nanosleep(backoff);
-        if (ld_acquire_u32(flag) == epoch) return true;
-        if (backoff < 1024) backoff <<= 1;
-        if (clock64() - start > TRI_WAIT_BOUND) {
-            const unsigned long long now = progress_sum(progress, n_progress);
-            if (have && now == seen) return false;
-            have = true;  // the solve moved (or this is the first look): wait on
-            seen = now;
-            start = clock64();
-        }
-    }
-}
-
 // UPPER: rows in descending order, terms col > r.  REV: the terms of a row are subtracted in
-// descending column order (usolve_csc).
-template <typename P, bool UPPER, bool REV>
+// descending column order (usolve_csc).  UNIT: the rows hold only the triangle's terms and the
+// diagonal is 1 (the L of an LDL^T factorization): no diagonal lookup, no division.
+template <typename P, bool UPPER, bool REV, bool UNIT = false>
 __global__ void __launch_bounds__(TRI_THREADS) trisolve_kernel(TriArgs<P> a) {
     const unsigned lane = threadIdx.x & 31;
     unsigned long long* mine = a.progress + blockIdx.x * (TRI_THREADS / 32) + threadIdx.x / 32;
@@ -158,11 +129,13 @@ __global__ void __launch_bounds__(TRI_THREADS) trisolve_kernel(TriArgs<P> a) {
         if (t >= a.n_work) return;
         const uint64_t r = UPPER ? a.n - 1 - t : t;
         const uint64_t s = a.ip[r], e = a.ip[r + 1];
-        const uint64_t d = s + a.diag[r];  // first position with col >= r
+        const uint64_t d = UNIT ? s : s + a.diag[r];  // first position with col >= r
         const bool solve = t < a.k_ticket;
         // the triangle's terms: [s, d) below the diagonal, (diagonal, e) above it
         uint64_t lo = s, hi = d;
-        if (UPPER) {
+        if (UNIT) {
+            hi = e;
+        } else if (UPPER) {
             lo = (d < e && a.idx[d] == r) ? d + 1 : d;
             hi = e;
         }
@@ -191,7 +164,7 @@ __global__ void __launch_bounds__(TRI_THREADS) trisolve_kernel(TriArgs<P> a) {
             if ((base + 32) % TRI_HEARTBEAT == 0 && lane == 0) __stcg(mine, ++done);
         }
         if (lane == 0) {
-            if (solve) x = __ddiv_rn(x, __ldg(a.val + d));
+            if (solve && !UNIT) x = __ddiv_rn(x, __ldg(a.val + d));
             __stcg(a.x + r, x);
             if (solve) st_release_u32(a.flags + r, a.epoch);
             __stcg(mine, ++done);
@@ -240,7 +213,11 @@ int launch_solve(sprs_b200_trisolve* p, double* d_x, cudaStream_t s) {
     a.n_progress = (uint64_t)g * warps_per_cta;
     SPRS_CUDA(ctx, cudaMemsetAsync(p->d_words, 0, sizeof(unsigned long long), s));
     SPRS_CUDA(ctx, cudaMemsetAsync(p->d_progress, 0, a.n_progress * sizeof(unsigned long long), s));
-    if (p->tri == SPRS_B200_TRI_LOWER)
+    if (p->unit && p->tri == SPRS_B200_TRI_LOWER)
+        trisolve_kernel<P, false, false, true><<<g, TRI_THREADS, 0, s>>>(a);
+    else if (p->unit)
+        trisolve_kernel<P, true, false, true><<<g, TRI_THREADS, 0, s>>>(a);
+    else if (p->tri == SPRS_B200_TRI_LOWER)
         trisolve_kernel<P, false, false><<<g, TRI_THREADS, 0, s>>>(a);
     else if (csc)
         trisolve_kernel<P, true, true><<<g, TRI_THREADS, 0, s>>>(a);
@@ -295,6 +272,21 @@ void free_plan(sprs_b200_trisolve* p) {
     delete p;
 }
 
+// the flags, counters and wait-bound words of a plan
+int alloc_solve_state(sprs_b200_trisolve* p, cudaStream_t s) {
+    sprs_b200_ctx* ctx = p->ctx;
+    const uint64_t n = p->n;
+    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_flags, n * sizeof(uint32_t) + 16));
+    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_words, 2 * sizeof(unsigned long long)));
+    p->n_progress = (uint64_t)ctx->sm_count * TRI_CTAS_PER_SM * (TRI_THREADS / 32);
+    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_progress, p->n_progress * sizeof(unsigned long long)));
+    SPRS_CUDA(ctx, cudaEventCreateWithFlags(&p->ev_last, cudaEventDisableTiming));
+    SPRS_CUDA(ctx, cudaMallocHost((void**)&p->h_err, sizeof(unsigned long long)));
+    *p->h_err = 0;
+    SPRS_CUDA(ctx, cudaMemsetAsync(p->d_flags, 0, n * sizeof(uint32_t) + 16, s));
+    return SPRS_B200_OK;
+}
+
 int build_plan(sprs_b200_trisolve* p, const sprs_b200_csmat* mat) {
     sprs_b200_ctx* ctx = p->ctx;
     cudaStream_t s = ctx->stream;
@@ -307,14 +299,7 @@ int build_plan(sprs_b200_trisolve* p, const sprs_b200_csmat* mat) {
     }
     const uint64_t n = p->n;
     SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_diag, n * sizeof(uint32_t) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_flags, n * sizeof(uint32_t) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_words, 2 * sizeof(unsigned long long)));
-    p->n_progress = (uint64_t)ctx->sm_count * TRI_CTAS_PER_SM * (TRI_THREADS / 32);
-    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_progress, p->n_progress * sizeof(unsigned long long)));
-    SPRS_CUDA(ctx, cudaEventCreateWithFlags(&p->ev_last, cudaEventDisableTiming));
-    SPRS_CUDA(ctx, cudaMallocHost((void**)&p->h_err, sizeof(unsigned long long)));
-    *p->h_err = 0;
-    SPRS_CUDA(ctx, cudaMemsetAsync(p->d_flags, 0, n * sizeof(uint32_t) + 16, s));
+    SPRS_TRY(alloc_solve_state(p, s));
     unsigned long long key = ~0ull;
     SPRS_CUDA(ctx, cudaMemcpyAsync(p->d_words + 1, &key, sizeof(key), cudaMemcpyHostToDevice, s));
     if (n) SPRS_TRY(p->csr->indptr_bytes == 4 ? launch_plan<uint32_t>(p, s) : launch_plan<uint64_t>(p, s));
@@ -335,6 +320,33 @@ int build_plan(sprs_b200_trisolve* p, const sprs_b200_csmat* mat) {
 }
 
 }  // namespace
+
+int trisolve_unit_plan(sprs_b200_ctx* ctx, const sprs_b200_csmat* csr, int tri,
+                       sprs_b200_trisolve** out) {
+    *out = nullptr;
+    auto* p = new sprs_b200_trisolve();
+    p->ctx = ctx;
+    p->csr = csr;
+    p->tri = tri;
+    p->n = csr->rows;
+    p->k_ticket = p->n;
+    p->unit = true;
+    const int st = alloc_solve_state(p, ctx->stream);
+    if (st != SPRS_B200_OK) {
+        free_plan(p);
+        return st;
+    }
+    *out = p;
+    return SPRS_B200_OK;
+}
+
+int trisolve_enqueue(sprs_b200_trisolve* plan, double* d_x, cudaStream_t s) {
+    return enqueue_solve(plan, d_x, s);
+}
+
+int trisolve_check_breach(sprs_b200_trisolve* plan) {
+    return take_breach(plan, "in this solve");
+}
 
 extern "C" {
 

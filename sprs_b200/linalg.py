@@ -9,6 +9,8 @@
 dense-rhs solves, bit-identical to the reference (csrc/trisolve.cu), and `TriSolvePlan` for
 repeated solves of one matrix and the device-resident form.
 
+`diag_solve` mirrors sprs::linalg::diag_solve.  The LDL^T factorization is in `sprs_b200.ldl`.
+
 Differences a caller can see in BiCGSTAB, both forced by the host language:
   * vectors are dense float64 arrays (a CsVec argument is densified; the reference's CsVec
     arithmetic is dense arithmetic on the union pattern, binop.rs:442-470), accessors return
@@ -292,6 +294,20 @@ class TriSolvePlan:
             pass
 
 
+def diag_solve(diag, x):
+    """sprs::linalg::diag_solve (sparse/linalg.rs): x (a contiguous, writeable float64 array)
+    divided in place by diag, entry by entry, on the device."""
+    from .sparse import Context
+    _check_rhs(x)
+    d = np.ascontiguousarray(diag, dtype=np.float64)
+    if d.ndim != 1 or d.size != x.size:
+        raise SprsPanic("assertion `left == right` failed\n  left: %d\n right: %d"
+                        % (d.size, x.size))
+    ctx = Context.default()
+    ctx.check(ctx.lib.sprs_b200_diag_solve(ctx.h, d.ctypes.data_as(C.c_void_p),
+                                           x.ctypes.data_as(C.c_void_p), x.size))
+
+
 def _check_rhs(rhs):
     if not (isinstance(rhs, np.ndarray) and rhs.dtype == np.float64 and rhs.ndim == 1 and
             rhs.flags.c_contiguous and rhs.flags.writeable):
@@ -343,4 +359,4 @@ class trisolve:  # noqa: N801  (module path of the reference: sprs::linalg::tris
         _dense_rhs_solve(upper_tri_mat, rhs, False, False)
 
 
-__all__ = ["BiCGSTAB", "NotConverged", "bicgstab", "TriSolvePlan", "trisolve"]
+__all__ = ["BiCGSTAB", "NotConverged", "bicgstab", "TriSolvePlan", "trisolve", "diag_solve"]

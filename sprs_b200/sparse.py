@@ -91,6 +91,8 @@ class Context:
         if st == _lib.ERR_SINGULAR:  # message: "Singular matrix at index {i} ({reason})"
             head, _, reason = msg.partition(" (")
             raise SingularMatrix(int(head.rsplit(" ", 1)[-1]), reason[:-1])
+        if st == _lib.ERR_NOT_SYMMETRIC:
+            raise SprsPanic(msg)
         raise ThirdPartyError(st, msg)
 
     def synchronize(self):
