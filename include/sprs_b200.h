@@ -133,6 +133,34 @@ int sprs_b200_csmat_binop(sprs_b200_ctx* ctx, const sprs_b200_csmat* lhs,
 int sprs_b200_csmat_scale(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, double s,
                           sprs_b200_csmat** out);
 
+/* ---- sparse matrix construction, device-resident result (construct.rs, kronecker.rs) -----
+ * bmat (construct.rs): a CSR mirror built from an n_block_rows x n_block_cols grid of blocks
+ * (row-major; NULL = None, i.e. zero(max rows of its block row, max cols of its block column)).
+ * Blocks may be CSR or CSC (a CSC block goes through its cached CSR conversion) with any mix of
+ * indptr widths.  The result is what the reference's hstack of every block row followed by the
+ * vstack of the rows gives.  Checks, in the reference's order, before any device work:
+ *   ERR_ARGUMENT    "Empty stacking list" (no block row or no block column), then
+ *                   "Empty bmat row", then "Empty bmat col";
+ *   ERR_DIMENSION   "Dimension mismatch": a present block whose row count is not its block
+ *                   row's, or block rows whose total widths (a None counting as its column's
+ *                   widest block) differ;
+ *   ERR_INDEX_RANGE a result dimension >= 2^32 (device mirrors index with u32).
+ * vstack(mats) is bmat with one block column; hstack(mats) is the transpose view of the vstack
+ * of the blocks' transpose views.  Blocking, ctx stream.                                       */
+int sprs_b200_csmat_bmat(sprs_b200_ctx* ctx, uint64_t n_block_rows, uint64_t n_block_cols,
+                         const sprs_b200_csmat* const* blocks, sprs_b200_csmat** out);
+/* kronecker_product (kronecker.rs): a new mirror in a's storage (b converted to a's storage
+ * first when they differ).  Output outer vector oa * outer(b) + ob lists, for each entry
+ * (ja, va) of a's vector oa, each entry (jb, vb) of b's vector ob: index ja * inner(b) + jb,
+ * value va * vb (one IEEE multiply, nothing dropped).  ERR_INDEX_RANGE when a result dimension
+ * is >= 2^32 or the shape or nnz(a) * nnz(b) overflows 64 bits.  Blocking, ctx stream.          */
+int sprs_b200_csmat_kron(sprs_b200_ctx* ctx, const sprs_b200_csmat* a, const sprs_b200_csmat* b,
+                         sprs_b200_csmat** out);
+/* transpose_view: a mirror of the same device arrays in the other storage with the shape
+ * swapped (no copy).  m must outlive the view; freeing the view leaves m's arrays alone.       */
+int sprs_b200_csmat_transpose_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m,
+                                   sprs_b200_csmat** out);
+
 /* ---- sparse x dense vector, HOST buffers (copies are part of the call) --------
  * prod::mul_acc_mat_vec_csr(mat, in_vec, res_vec)  prod.rs:103-127 : y += A x
  * prod::mul_acc_mat_vec_csc                        prod.rs:74-99

@@ -433,6 +433,121 @@ CsMatI<I, Iptr> operator*(const CsMatI<I, Iptr>& a, double s) {
     sprs_b200_csmat_free(c);
     return out;
 }
+// ---- bmat / vstack / hstack (construct.rs) and kronecker_product (kronecker.rs) on the device.
+// Results are bit-identical to the reference; a result dimension >= 2^32 panics (device
+// mirrors index with u32) even where usize would allow it.  Blocks are pointers, nullptr = None.
+namespace detail {
+inline sprs_b200_csmat* bmat_dev(Context& ctx, size_t n_rows, size_t n_cols,
+                                 const std::vector<const sprs_b200_csmat*>& grid) {
+    sprs_b200_csmat* c = nullptr;
+    ctx.check(sprs_b200_csmat_bmat(ctx.handle(), n_rows, n_cols, grid.data(), &c));
+    return c;
+}
+}  // namespace detail
+
+// bmat: the asserts in the reference's order, then the device concatenation (always CSR)
+template <class I, class Iptr>
+CsMatI<I, Iptr> bmat(const std::vector<std::vector<const CsMatI<I, Iptr>*>>& blocks) {
+    if (blocks.empty() || blocks[0].empty()) throw Panic("Empty stacking list");
+    const size_t nbr = blocks.size(), nbc = blocks[0].size();
+    for (const auto& row : blocks)
+        if (row.size() != nbc) throw Panic("Dimension mismatch");
+    for (const auto& row : blocks) {
+        bool any = false;
+        for (const auto* m : row) any = any || m;
+        if (!any) throw Panic("Empty bmat row");
+    }
+    std::vector<size_t> widths(nbc, 0);
+    for (size_t j = 0; j < nbc; ++j) {
+        bool any = false;
+        for (const auto& row : blocks)
+            if (row[j]) {
+                any = true;
+                widths[j] = std::max(widths[j], row[j]->cols());
+            }
+        if (!any) throw Panic("Empty bmat col");
+    }
+    Context& ctx = Context::thread_default();
+    std::vector<const sprs_b200_csmat*> grid;
+    size_t rows = 0, cols = 0;
+    for (size_t i = 0; i < nbr; ++i) {
+        size_t height = 0;
+        for (size_t j = 0; j < nbc; ++j) {
+            const auto* m = blocks[i][j];
+            grid.push_back(m ? m->device() : nullptr);
+            if (m) height = std::max(height, m->rows());
+            if (i == 0) cols += m ? m->cols() : widths[j];
+        }
+        rows += height;
+    }
+    sprs_b200_csmat* c = detail::bmat_dev(ctx, nbr, nbc, grid);
+    CsMatI<I, Iptr> out = CsMatI<I, Iptr>::download(ctx, c, CSR, rows, cols);
+    sprs_b200_csmat_free(c);
+    return out;
+}
+
+// vstack: the CSR forms stacked vertically (always CSR)
+template <class I, class Iptr>
+CsMatI<I, Iptr> vstack(const std::vector<CsMatI<I, Iptr>>& mats) {
+    if (mats.empty()) throw Panic("Empty stacking list");
+    std::vector<std::vector<const CsMatI<I, Iptr>*>> col;
+    for (const auto& m : mats) col.push_back({&m});
+    return bmat(col);
+}
+
+// hstack: the CSC forms stacked horizontally (always CSC) -- on the device, the vstack of the
+// blocks' transpose views, read back as the CSC it is
+template <class I, class Iptr>
+CsMatI<I, Iptr> hstack(const std::vector<CsMatI<I, Iptr>>& mats) {
+    if (mats.empty()) throw Panic("Empty stacking list");
+    Context& ctx = Context::thread_default();
+    std::vector<const sprs_b200_csmat*> views;
+    size_t cols = 0;
+    int st = SPRS_B200_OK;
+    for (const auto& m : mats) {
+        sprs_b200_csmat* v = nullptr;
+        if ((st = sprs_b200_csmat_transpose_view(ctx.handle(), m.device(), &v)) != SPRS_B200_OK)
+            break;
+        views.push_back(v);
+        cols += m.cols();
+    }
+    sprs_b200_csmat* c = nullptr;
+    if (st == SPRS_B200_OK) st = sprs_b200_csmat_bmat(ctx.handle(), views.size(), 1, views.data(), &c);
+    for (const auto* v : views) sprs_b200_csmat_free(const_cast<sprs_b200_csmat*>(v));
+    ctx.check(st);
+    CsMatI<I, Iptr> out = CsMatI<I, Iptr>::download(ctx, c, CSC, mats[0].rows(), cols);
+    sprs_b200_csmat_free(c);
+    return out;
+}
+
+// kronecker_product: in a's storage, b converted when the storages differ.  A produced index
+// that does not fit I panics like the reference's `I::from(..).unwrap()`.
+template <class I, class Iptr>
+CsMatI<I, Iptr> kronecker_product(const CsMatI<I, Iptr>& a, const CsMatI<I, Iptr>& b) {
+    if (a.nnz() && b.nnz()) {
+        auto max_inner = [&](const CsMatI<I, Iptr>& m) -> uint64_t {  // in a's storage
+            uint64_t top = 0;
+            for (size_t o = 0; o < m.outer_dims(); ++o)
+                if (m.indptr()[o + 1] > m.indptr()[o])
+                    top = m.storage() == a.storage()
+                              ? std::max<uint64_t>(top, (uint64_t)m.indices()[(size_t)(m.indptr()[o + 1] - m.indptr()[0]) - 1])
+                              : o;
+            return top;
+        };
+        const uint64_t inner_b = b.storage() == a.storage() ? b.inner_dims() : b.outer_dims();
+        const unsigned __int128 top = (unsigned __int128)max_inner(a) * inner_b + max_inner(b);
+        if (top > (unsigned __int128)(uint64_t)std::numeric_limits<I>::max())
+            throw Panic("called `Option::unwrap()` on a `None` value");
+    }
+    Context& ctx = Context::thread_default();
+    sprs_b200_csmat* c = nullptr;
+    ctx.check(sprs_b200_csmat_kron(ctx.handle(), a.device(), b.device(), &c));
+    CsMatI<I, Iptr> out = CsMatI<I, Iptr>::download(ctx, c, a.storage(), a.rows() * b.rows(),
+                                                    a.cols() * b.cols());
+    sprs_b200_csmat_free(c);
+    return out;
+}
+
 // `&A * &x`, x: Array1 (csmat.rs:2119-2160)
 template <class I, class Iptr>
 Array1 operator*(const CsMatI<I, Iptr>& a, const Array1& x) {

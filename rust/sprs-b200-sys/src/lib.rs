@@ -68,6 +68,15 @@ extern "C" {
     pub fn sprs_b200_csmat_scale(
         ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat, s: c_double,
         out: *mut *mut sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_csmat_bmat(
+        ctx: *mut sprs_b200_ctx, n_block_rows: u64, n_block_cols: u64,
+        blocks: *const *const sprs_b200_csmat, out: *mut *mut sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_csmat_kron(
+        ctx: *mut sprs_b200_ctx, a: *const sprs_b200_csmat, b: *const sprs_b200_csmat,
+        out: *mut *mut sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_csmat_transpose_view(
+        ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat,
+        out: *mut *mut sprs_b200_csmat) -> c_int;
     pub fn sprs_b200_mul_acc_mat_vec_csr(
         ctx: *mut sprs_b200_ctx, mat: *const sprs_b200_csmat, in_vec: *const c_double, in_len: u64,
         res_vec: *mut c_double, res_len: u64) -> c_int;

@@ -245,6 +245,114 @@ pub mod binop {
     }
 }
 
+/// sprs::bmat / vstack / hstack (construct.rs) and sprs::kronecker_product (kronecker.rs) on the
+/// device, bit-identical to the reference (csrc/construct.cu).  The asserts run here in the
+/// reference's order; a result dimension >= 2^32 is a device error (u32 mirrors) even where
+/// usize would allow it.
+pub mod construct {
+    use super::*;
+    use sprs::CompressedStorage::{CSC, CSR};
+
+    fn download_as<I: SpIndex, Iptr: SpIndex>(c: *mut ffi::sprs_b200_ctx, m: *mut ffi::sprs_b200_csmat,
+                                              storage: sprs::CompressedStorage,
+                                              shape: (usize, usize)) -> CsMatI<f64, I, Iptr> {
+        let outer = if storage == CSR { shape.0 } else { shape.1 };
+        let nnz = unsafe { ffi::sprs_b200_csmat_nnz(m) } as usize;
+        let mut indptr = vec![Iptr::zero(); outer + 1];
+        let mut indices = vec![I::zero(); nnz];
+        let mut data = vec![0f64; nnz];
+        let st = unsafe {
+            ffi::sprs_b200_csmat_download(c, m, indptr.as_mut_ptr() as *mut c_void,
+                std::mem::size_of::<Iptr>() as i32, indices.as_mut_ptr() as *mut c_void,
+                std::mem::size_of::<I>() as i32, data.as_mut_ptr())
+        };
+        unsafe { ffi::sprs_b200_csmat_free(m); }
+        check(c, st).expect("sprs_b200 device error");
+        // sorted unique in-range indices by construction
+        CsMatI::new_trusted(storage, shape, indptr, indices, data)
+    }
+
+    /// bmat (construct.rs): always CSR; `None` is zero((max rows of its block row, max cols of
+    /// its block column)).
+    pub fn bmat<I: SpIndex, Iptr: SpIndex>(blocks: &[Vec<Option<&DeviceCsMat<I, Iptr>>>]) -> CsMatI<f64, I, Iptr> {
+        assert_ne!(blocks.len(), 0, "Empty stacking list");
+        let nbc = blocks[0].len();
+        assert_ne!(nbc, 0, "Empty stacking list");
+        assert!(blocks.iter().all(|r| r.len() == nbc), "Dimension mismatch");
+        assert!(!blocks.iter().any(|r| r.iter().all(Option::is_none)), "Empty bmat row");
+        assert!(!(0..nbc).any(|j| blocks.iter().all(|r| r[j].is_none())), "Empty bmat col");
+        let widths: Vec<usize> = (0..nbc)
+            .map(|j| blocks.iter().filter_map(|r| r[j].map(|m| m.host.cols())).max().unwrap_or(0))
+            .collect();
+        let rows: usize = blocks.iter()
+            .map(|r| r.iter().filter_map(|m| m.map(|m| m.host.rows())).max().unwrap_or(0)).sum();
+        let cols: usize = blocks[0].iter().zip(&widths).map(|(m, w)| m.map_or(*w, |m| m.host.cols())).sum();
+        let grid: Vec<*const ffi::sprs_b200_csmat> = blocks.iter()
+            .flat_map(|r| r.iter().map(|m| m.map_or(std::ptr::null(), |m| m.dev as *const _)))
+            .collect();
+        CTX.with(|c| {
+            let mut out = std::ptr::null_mut();
+            check(c.0, unsafe { ffi::sprs_b200_csmat_bmat(c.0, blocks.len() as u64, nbc as u64, grid.as_ptr(), &mut out) })
+                .expect("sprs_b200 device error");
+            download_as(c.0, out, CSR, (rows, cols))
+        })
+    }
+
+    /// vstack (construct.rs): the CSR forms stacked vertically; always CSR.
+    pub fn vstack<I: SpIndex, Iptr: SpIndex>(mats: &[&DeviceCsMat<I, Iptr>]) -> CsMatI<f64, I, Iptr> {
+        assert!(!mats.is_empty(), "Empty stacking list");
+        let col: Vec<Vec<Option<&DeviceCsMat<I, Iptr>>>> = mats.iter().map(|m| vec![Some(*m)]).collect();
+        bmat(&col)
+    }
+
+    /// hstack (construct.rs): the CSC forms stacked horizontally; always CSC.  On the device it
+    /// is the vstack of the blocks' transpose views, read back as the CSC it is.
+    pub fn hstack<I: SpIndex, Iptr: SpIndex>(mats: &[&DeviceCsMat<I, Iptr>]) -> CsMatI<f64, I, Iptr> {
+        assert!(!mats.is_empty(), "Empty stacking list");
+        CTX.with(|c| {
+            let mut views: Vec<*const ffi::sprs_b200_csmat> = Vec::with_capacity(mats.len());
+            let mut st = ffi::SPRS_B200_OK;
+            for m in mats {
+                let mut v = std::ptr::null_mut();
+                st = unsafe { ffi::sprs_b200_csmat_transpose_view(c.0, m.dev, &mut v) };
+                if st != ffi::SPRS_B200_OK { break; }
+                views.push(v);
+            }
+            let mut out = std::ptr::null_mut();
+            if st == ffi::SPRS_B200_OK {
+                st = unsafe { ffi::sprs_b200_csmat_bmat(c.0, views.len() as u64, 1, views.as_ptr(), &mut out) };
+            }
+            for v in views { unsafe { ffi::sprs_b200_csmat_free(v as *mut _); } }
+            check(c.0, st).expect("sprs_b200 device error");
+            let cols = mats.iter().map(|m| m.host.cols()).sum();
+            download_as(c.0, out, CSC, (mats[0].host.rows(), cols))
+        })
+    }
+
+    /// kronecker_product (kronecker.rs): in a's storage, b converted when the storages differ;
+    /// a produced index that does not fit I panics like the reference's `unwrap()`.
+    pub fn kronecker_product<I: SpIndex, Iptr: SpIndex>(a: &DeviceCsMat<I, Iptr>, b: &DeviceCsMat<I, Iptr>) -> CsMatI<f64, I, Iptr> {
+        let (ha, hb) = (&a.host, &b.host);
+        if ha.nnz() > 0 && hb.nnz() > 0 {
+            let max_a = ha.indices().iter().map(|i| i.index()).max().unwrap_or(0);
+            let (inner_b, max_b) = if hb.storage() == ha.storage() {
+                (hb.inner_dims(), hb.indices().iter().map(|i| i.index()).max().unwrap_or(0))
+            } else {
+                let last = hb.indptr().to_proper().windows(2).rposition(|w| w[1] > w[0]).unwrap_or(0);
+                (hb.outer_dims(), last)
+            };
+            let top = (max_a as u128) * (inner_b as u128) + max_b as u128;
+            assert!(top <= I::max_value().index() as u128, "called `Option::unwrap()` on a `None` value");
+        }
+        CTX.with(|c| {
+            let mut out = std::ptr::null_mut();
+            check(c.0, unsafe { ffi::sprs_b200_csmat_kron(c.0, a.dev, b.dev, &mut out) })
+                .expect("sprs_b200 device error");
+            download_as(c.0, out, ha.storage(), (ha.rows() * hb.rows(), ha.cols() * hb.cols()))
+        })
+    }
+}
+
 /// sprs::linalg::bicgstab::BiCGSTAB<f64> (linalg/bicgstab.rs:95-300) with x, r, rhat, p
 /// resident on the device between iterations.  Same constructor, `solve`, `step`,
 /// restarts and accessors; vectors cross the API as dense `Array1<f64>`.

@@ -5,14 +5,17 @@ Nothing here computes on the CPU: every product is a call into libsprs_b200.so
 (hand-written CUDA).  Importing works without a GPU (so the ABI can be inspected);
 creating a Context without one raises ThirdPartyError.
 """
-from . import _lib, io, ldl, linalg
+from . import _lib, construct, io, ldl, linalg
+from .construct import bmat, hstack, kronecker_product, vstack
 from .ldl import is_symmetric
 from .sparse import (CSC, CSR, Context, CsMat, CsVec, DeviceCsMat, SingularMatrix, SprsPanic,
                      ThirdPartyError, binop, csmat_mul_csmat, prod, smmp)
 
 __all__ = ["CSC", "CSR", "Context", "CsMat", "CsVec", "DeviceCsMat", "SingularMatrix", "SprsPanic",
-           "ThirdPartyError", "binop", "csmat_mul_csmat", "is_symmetric", "prod", "smmp", "_lib", "io",
-           "ldl", "linalg"]
+           "ThirdPartyError", "binop", "bmat", "construct", "csmat_mul_csmat", "hstack",
+           "is_symmetric", "kronecker_product", "prod", "smmp", "vstack", "_lib", "io", "ldl",
+           "linalg"]
+CONSTRUCT_TILE = 2048  # output entries per warp tile of the construction kernels (csrc/construct.cu)
 __version__ = "0.1.0"
 import os as _os
 

@@ -51,6 +51,9 @@ PROTOTYPES = {
     "sprs_b200_csmat_to_other_storage": (_int, [_vp, _vp, C.POINTER(_vp)]),
     "sprs_b200_csmat_binop": (_int, [_vp, _vp, _vp, _int, C.POINTER(_vp)]),
     "sprs_b200_csmat_scale": (_int, [_vp, _vp, C.c_double, C.POINTER(_vp)]),
+    "sprs_b200_csmat_bmat": (_int, [_vp, _u64, _u64, C.POINTER(_vp), C.POINTER(_vp)]),
+    "sprs_b200_csmat_kron": (_int, [_vp, _vp, _vp, C.POINTER(_vp)]),
+    "sprs_b200_csmat_transpose_view": (_int, [_vp, _vp, C.POINTER(_vp)]),
     "sprs_b200_mul_acc_mat_vec_csr": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
     "sprs_b200_mul_acc_mat_vec_csc": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
     "sprs_b200_mul_mat_vec": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
@@ -144,7 +147,9 @@ _NOT_EMULATED = ("sprs_b200_comm_", "sprs_b200_symm_", "sprs_b200_partition_rows
                  # so are the triangular solves (tests/emu_trisolve.py)
                  "sprs_b200_trisolve_",
                  # and the LDL^T factorization (tests/emu_ldl.py)
-                 "sprs_b200_ldl_", "sprs_b200_is_symmetric", "sprs_b200_diag_solve")
+                 "sprs_b200_ldl_", "sprs_b200_is_symmetric", "sprs_b200_diag_solve",
+                 # and the construction (tests/emu_construct.py)
+                 "sprs_b200_csmat_bmat", "sprs_b200_csmat_kron", "sprs_b200_csmat_transpose_view")
 _lib = None
 
 

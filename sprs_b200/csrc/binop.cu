@@ -225,6 +225,9 @@ __global__ void scale_kernel(const P* __restrict__ ip, const uint32_t* __restric
         ip_out[i] = ip[i];
 }
 
+}  // namespace
+
+// ---- result helpers, shared with construct.cu (declared in common.cuh)
 bool force_indptr64() {
     // the SPRS_B200_FORCE_INDPTR64 test hook of csmat_upload, applied to the results too
     static const bool force64 = [] {
@@ -266,6 +269,8 @@ int finish_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, const 
         SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "%s: kernel failed", what);
     return SPRS_B200_OK;
 }
+
+namespace {
 
 template <typename PA, typename PB, typename PC>
 void launch_fill(const Operands<PA, PB>& o, int op, uint64_t total, uint64_t n_tiles,

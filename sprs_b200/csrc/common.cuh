@@ -151,6 +151,17 @@ int transpose_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, sprs_b200_csm
 // device conversion, owned by the mirror (api.cu)
 int csmat_csr_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const sprs_b200_csmat** out);
 
+// ---- device-built results (binop.cu; the binops, scale and construct.cu use them)
+// the SPRS_B200_FORCE_INDPTR64 test hook of csmat_upload, applied to the results too
+bool force_indptr64();
+// a pooled result mirror with like's storage and shape (no arrays yet)
+sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, const sprs_b200_csmat* like, uint64_t nnz,
+                            int indptr_bytes);
+// its indptr / indices / data, stream-ordered on s
+int alloc_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s);
+// its SpMV partition (no hot set), then wait for s
+int finish_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, const char* what);
+
 // ---- small device helpers -----------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

@@ -324,3 +324,24 @@ def scale(ctx, a, s):
     cm = C.c_void_p()
     ctx.check(ctx.lib.sprs_b200_csmat_scale(ctx.h, ma.h, float(s), C.byref(cm)))
     return _with_views(ctx, DeviceCsMat(ctx, cm))
+
+
+def bmat(ctx, blocks):
+    """sprs::bmat on the device (csrc/construct.cu): blocks is a list of rows of DeviceCsr,
+    DeviceCsMat or None.  Returns (mirror, indptr, indices, data) of the CSR result like binop."""
+    from .construct import bmat_dev
+    if _device(ctx).type == "cuda":
+        _sync()  # blocks produced on torch's stream; the construction runs on the ctx stream
+    mirrors = [[b.mirror if isinstance(b, DeviceCsr) else b for b in row] for row in blocks]
+    return _with_views(ctx, bmat_dev(ctx, mirrors))
+
+
+def kron(ctx, a, b):
+    """sprs::kronecker_product on the device (csrc/construct.cu), in a's storage; returns
+    (mirror, indptr, indices, data) like binop."""
+    from .construct import kron_dev
+    ma = a.mirror if isinstance(a, DeviceCsr) else a
+    mb = b.mirror if isinstance(b, DeviceCsr) else b
+    if _device(ctx).type == "cuda":
+        _sync()
+    return _with_views(ctx, kron_dev(ctx, ma, mb))
