@@ -161,6 +161,54 @@ int sprs_b200_csmat_kron(sprs_b200_ctx* ctx, const sprs_b200_csmat* a, const spr
 int sprs_b200_csmat_transpose_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m,
                                    sprs_b200_csmat** out);
 
+/* ---- the dense boundary (to_dense.rs, csmat.rs:502-549, binop.rs:273-433) --------------------
+ * Dense operands are (pointer, rows, cols, rs, cs): element (r, c) at p[r * rs + c * cs], with
+ * signed element strides (any ndarray view: negative, zero and non-unit strides work).  The
+ * host-buffer forms block and pass views through the pinned staging buffer; the _dev forms take
+ * device pointers and run on `stream` (NULL = legacy default stream).
+ * to_dense (csmat.rs:1127-1134): out is C order with leading dimension ld >= cols (else
+ * DIMENSION); stored values copied as bits, +0.0 everywhere else, for CSR and CSC alike.        */
+int sprs_b200_csmat_to_dense(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, double* out,
+                             uint64_t ld);
+int sprs_b200_csmat_to_dense_dev(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, double* d_out,
+                                 uint64_t ld, void* stream);
+/* assign_to_dense (to_dense.rs:12-30): out(r, c) = value of every stored entry, as bits; every
+ * other element untouched.  DIMENSION if cols or rows differ.  Device work O(nnz + outer).     */
+int sprs_b200_assign_to_dense(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, double* out,
+                              uint64_t rows, uint64_t cols, int64_t rs, int64_t cs);
+int sprs_b200_assign_to_dense_dev(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, double* d_out,
+                                  uint64_t rows, uint64_t cols, int64_t rs, int64_t cs,
+                                  void* stream);
+/* csr_from_dense / csc_from_dense (csmat.rs:502-549): a new device mirror in `storage` holding
+ * every x with |x| > eps', eps' = epsilon if epsilon > 0 else +0.0 (so +-0 and NaN are never
+ * kept), the value copied as bits; inner indices ascend in each outer vector.  INDEX_RANGE if a
+ * dimension is >= 2^32; 64-bit indptr when nnz >= 2^32 - 1.  Blocking, ctx stream (a _dev
+ * operand must be complete when called).                                                       */
+int sprs_b200_csmat_from_dense(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
+                               const double* m, int64_t rs, int64_t cs, double epsilon,
+                               sprs_b200_csmat** out);
+int sprs_b200_csmat_from_dense_dev(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
+                                   const double* d_m, int64_t rs, int64_t cs, double epsilon,
+                                   sprs_b200_csmat** out);
+/* csmat_binop_dense_raw (binop.rs:384-433) with the closures of add_dense_mat_same_ordering
+ * (op ADD: alpha*x + beta*y) and mul_dense_mat_same_ordering (op MUL: alpha*x*y, beta ignored),
+ * each operation rounded on its own; x = +0.0 where lhs has no entry.  Every out element is
+ * written; out may be rhs itself (same pointer and strides).  Checks, in order: DIMENSION (any of
+ * the four shape equalities), STORAGE unless (CSR, rhs and out with Axis(1) fastest) or (CSC,
+ * both with Axis(0) fastest), where Axis(0) is fastest iff cs > rs; then ARGUMENT for SUB or an
+ * unknown op (the reference has no dense subtraction).                                          */
+int sprs_b200_csmat_binop_dense(sprs_b200_ctx* ctx, const sprs_b200_csmat* lhs, int op,
+                                double alpha, double beta, const double* rhs, uint64_t rhs_rows,
+                                uint64_t rhs_cols, int64_t rhs_rs, int64_t rhs_cs, double* out,
+                                uint64_t out_rows, uint64_t out_cols, int64_t out_rs,
+                                int64_t out_cs);
+int sprs_b200_csmat_binop_dense_dev(sprs_b200_ctx* ctx, const sprs_b200_csmat* lhs, int op,
+                                    double alpha, double beta, const double* d_rhs,
+                                    uint64_t rhs_rows, uint64_t rhs_cols, int64_t rhs_rs,
+                                    int64_t rhs_cs, double* d_out, uint64_t out_rows,
+                                    uint64_t out_cols, int64_t out_rs, int64_t out_cs,
+                                    void* stream);
+
 /* ---- sparse x dense vector, HOST buffers (copies are part of the call) --------
  * prod::mul_acc_mat_vec_csr(mat, in_vec, res_vec)  prod.rs:103-127 : y += A x
  * prod::mul_acc_mat_vec_csc                        prod.rs:74-99

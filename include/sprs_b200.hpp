@@ -10,6 +10,8 @@
 //   sprs::prod::mul_acc_mat_vec_csr / csr_mulacc_dense_{row,col}maj / ...   prod.rs
 //   sprs::smmp::mul_csr_csr                            smmp.rs:196-237
 //   &a + &b, &a - &b, &a * s, binop::mul_mat_same_storage   binop.rs:20-163
+//   to_dense, assign_to_dense, csr/csc_from_dense, &a + &d,
+//   binop::{add,mul}_dense_mat_same_ordering   to_dense.rs, csmat.rs:502-549, binop.rs:273-433
 //
 // Contract violations throw sprs::Panic carrying the reference's panic message
 // ("Dimension mismatch", "Storage mismatch"; Guidelines.rst:9-27); device failures
@@ -257,6 +259,20 @@ class CsMatI {
         return CsMatI(st, {rows, cols}, std::move(ip), std::move(ind), std::move(d), 0);
     }
 
+    // to_dense (csmat.rs:1127-1134) on the device: C order, stored values as bits, +0.0 elsewhere
+    Array2 to_dense() const {
+        Array2 out = Array2::zeros(rows_, cols_);
+        if (rows_ && cols_) {
+            Context& ctx = Context::thread_default();
+            ctx.check(sprs_b200_csmat_to_dense(ctx.handle(), device(), out.data.data(), cols_));
+        }
+        return out;
+    }
+    // csr_from_dense / csc_from_dense (csmat.rs:502-549) on the device: |x| > epsilon kept
+    // (epsilon clamped to +0.0 unless > 0), values copied as bits
+    static CsMatI csr_from_dense(const Array2& m, double epsilon) { return from_dense(m, epsilon, CSR); }
+    static CsMatI csc_from_dense(const Array2& m, double epsilon) { return from_dense(m, epsilon, CSC); }
+
     double to_dense_at(size_t r, size_t c) const {
         const size_t o = is_csr() ? r : c, in = is_csr() ? c : r;
         for (size_t k = (size_t)(indptr_[o] - indptr_[0]); k < (size_t)(indptr_[o + 1] - indptr_[0]); ++k)
@@ -269,6 +285,17 @@ class CsMatI {
     auto dot(const R& rhs) const { return *this * rhs; }
 
    private:
+    static CsMatI from_dense(const Array2& m, double epsilon, CompressedStorage st) {
+        Context& ctx = Context::thread_default();
+        sprs_b200_csmat* t = nullptr;
+        const bool empty = m.rows == 0 || m.cols == 0;
+        ctx.check(sprs_b200_csmat_from_dense(ctx.handle(), st == CSR ? SPRS_B200_CSR : SPRS_B200_CSC,
+                                             m.rows, m.cols, empty ? nullptr : m.data.data(),
+                                             empty ? 0 : m.rs, empty ? 0 : m.cs, epsilon, &t));
+        CsMatI out = download(ctx, t, st, m.rows, m.cols);
+        sprs_b200_csmat_free(t);
+        return out;
+    }
     CsMatI(CompressedStorage st, std::pair<size_t, size_t> shape, std::vector<Iptr> ip,
            std::vector<I> ind, std::vector<double> d, int /*trusted*/)
         : storage_(st), rows_(shape.first), cols_(shape.second), indptr_(std::move(ip)),
@@ -433,6 +460,66 @@ CsMatI<I, Iptr> operator*(const CsMatI<I, Iptr>& a, double s) {
     sprs_b200_csmat_free(c);
     return out;
 }
+// ---- the dense boundary: to_dense.rs, binop.rs:273-433, csmat.rs:1951-1987
+namespace detail {
+// element strides as ndarray has them: an array with a zero-length axis has all-zero strides
+inline std::pair<std::ptrdiff_t, std::ptrdiff_t> nd_strides(const Array2& a) {
+    if (a.rows == 0 || a.cols == 0) return {0, 0};
+    return {a.rs, a.cs};
+}
+// utils::fastest_axis (sparse.rs:400-406): Axis(0) iff strides[1] > strides[0]
+inline int fastest_axis(const Array2& a) {
+    const auto st = nd_strides(a);
+    return st.second > st.first ? 0 : 1;
+}
+inline void binop_dense(const sprs_b200_csmat* lhs, int op, double alpha, double beta,
+                        const Array2& rhs, Array2& out) {
+    Context& ctx = Context::thread_default();
+    const auto r = nd_strides(rhs), o = nd_strides(out);
+    ctx.check(sprs_b200_csmat_binop_dense(ctx.handle(), lhs, op, alpha, beta, rhs.data.data(),
+                                          rhs.rows, rhs.cols, r.first, r.second, out.data.data(),
+                                          out.rows, out.cols, o.first, o.second));
+}
+}  // namespace detail
+
+// assign_to_dense (to_dense.rs:12-30): stored values into array as bits, the rest untouched
+template <class I, class Iptr>
+void assign_to_dense(Array2& array, const CsMatI<I, Iptr>& m) {
+    if (m.cols() != array.cols || m.rows() != array.rows) throw Panic("Dimension mismatch");
+    Context& ctx = Context::thread_default();
+    const auto st = detail::nd_strides(array);
+    ctx.check(sprs_b200_assign_to_dense(ctx.handle(), m.device(), array.data.data(), array.rows,
+                                        array.cols, st.first, st.second));
+}
+
+namespace binop {
+// add_dense_mat_same_ordering (binop.rs:279-323): (alpha*x) + (beta*y), x = +0.0 where lhs has
+// no entry; C order when rhs's fastest axis is Axis(1), F order otherwise
+template <class I, class Iptr>
+Array2 add_dense_mat_same_ordering(const CsMatI<I, Iptr>& lhs, const Array2& rhs, double alpha,
+                                   double beta) {
+    Array2 out = sprs::detail::fastest_axis(rhs) == 1 ? Array2::zeros(rhs.rows, rhs.cols)
+                                                : Array2::zeros_f(rhs.rows, rhs.cols);
+    sprs::detail::binop_dense(lhs.device(), SPRS_B200_BINOP_ADD, alpha, beta, rhs, out);
+    return out;
+}
+// mul_dense_mat_same_ordering (binop.rs:331-371): (alpha*x)*y
+template <class I, class Iptr>
+Array2 mul_dense_mat_same_ordering(const CsMatI<I, Iptr>& lhs, const Array2& rhs, double alpha) {
+    Array2 out = sprs::detail::fastest_axis(rhs) == 1 ? Array2::zeros(rhs.rows, rhs.cols)
+                                                : Array2::zeros_f(rhs.rows, rhs.cols);
+    sprs::detail::binop_dense(lhs.device(), SPRS_B200_BINOP_MUL, alpha, 0.0, rhs, out);
+    return out;
+}
+}  // namespace binop
+
+// `&A + &D` (csmat.rs:1951-1987): A converted first when its storage does not match D's layout
+template <class I, class Iptr>
+Array2 operator+(const CsMatI<I, Iptr>& a, const Array2& d) {
+    if (a.is_csr() == (detail::fastest_axis(d) == 1)) return binop::add_dense_mat_same_ordering(a, d, 1.0, 1.0);
+    return binop::add_dense_mat_same_ordering(a.to_other_storage(), d, 1.0, 1.0);
+}
+
 // ---- bmat / vstack / hstack (construct.rs) and kronecker_product (kronecker.rs) on the device.
 // Results are bit-identical to the reference; a result dimension >= 2^32 panics (device
 // mirrors index with u32) even where usize would allow it.  Blocks are pointers, nullptr = None.

@@ -77,6 +77,33 @@ extern "C" {
     pub fn sprs_b200_csmat_transpose_view(
         ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat,
         out: *mut *mut sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_csmat_to_dense(
+        ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat, out: *mut c_double, ld: u64) -> c_int;
+    pub fn sprs_b200_csmat_to_dense_dev(
+        ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat, d_out: *mut c_double, ld: u64,
+        stream: *mut c_void) -> c_int;
+    pub fn sprs_b200_assign_to_dense(
+        ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat, out: *mut c_double, rows: u64,
+        cols: u64, rs: i64, cs: i64) -> c_int;
+    pub fn sprs_b200_assign_to_dense_dev(
+        ctx: *mut sprs_b200_ctx, m: *const sprs_b200_csmat, d_out: *mut c_double, rows: u64,
+        cols: u64, rs: i64, cs: i64, stream: *mut c_void) -> c_int;
+    pub fn sprs_b200_csmat_from_dense(
+        ctx: *mut sprs_b200_ctx, storage: c_int, rows: u64, cols: u64, m: *const c_double,
+        rs: i64, cs: i64, epsilon: c_double, out: *mut *mut sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_csmat_from_dense_dev(
+        ctx: *mut sprs_b200_ctx, storage: c_int, rows: u64, cols: u64, d_m: *const c_double,
+        rs: i64, cs: i64, epsilon: c_double, out: *mut *mut sprs_b200_csmat) -> c_int;
+    pub fn sprs_b200_csmat_binop_dense(
+        ctx: *mut sprs_b200_ctx, lhs: *const sprs_b200_csmat, op: c_int, alpha: c_double,
+        beta: c_double, rhs: *const c_double, rhs_rows: u64, rhs_cols: u64, rhs_rs: i64,
+        rhs_cs: i64, out: *mut c_double, out_rows: u64, out_cols: u64, out_rs: i64,
+        out_cs: i64) -> c_int;
+    pub fn sprs_b200_csmat_binop_dense_dev(
+        ctx: *mut sprs_b200_ctx, lhs: *const sprs_b200_csmat, op: c_int, alpha: c_double,
+        beta: c_double, d_rhs: *const c_double, rhs_rows: u64, rhs_cols: u64, rhs_rs: i64,
+        rhs_cs: i64, d_out: *mut c_double, out_rows: u64, out_cols: u64, out_rs: i64,
+        out_cs: i64, stream: *mut c_void) -> c_int;
     pub fn sprs_b200_mul_acc_mat_vec_csr(
         ctx: *mut sprs_b200_ctx, mat: *const sprs_b200_csmat, in_vec: *const c_double, in_len: u64,
         res_vec: *mut c_double, res_len: u64) -> c_int;

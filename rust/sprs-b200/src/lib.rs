@@ -245,6 +245,106 @@ pub mod binop {
     }
 }
 
+/// The dense boundary on the device (the dense section of csrc/transpose.cu): to_dense.rs, CsMat::csr_from_dense /
+/// csc_from_dense (csmat.rs:502-549) and the sparse (+) dense half of binop.rs, bit-identical
+/// to the reference.  Views of any strides are passed as (pointer, shape, element strides);
+/// ndarray gives a view with a zero-length axis all-zero strides, and so does this crate.
+pub mod dense {
+    use super::*;
+    use ndarray::{Array2, ArrayBase, ArrayViewMut2, Data, Ix2, ShapeBuilder};
+
+    fn strides<S: ndarray::RawData>(a: &ArrayBase<S, Ix2>) -> (i64, i64) {
+        if a.is_empty() { (0, 0) } else { (a.strides()[0] as i64, a.strides()[1] as i64) }
+    }
+    fn c_like<S: ndarray::RawData>(a: &ArrayBase<S, Ix2>) -> bool {
+        let (rs, cs) = strides(a);
+        !(cs > rs)  // utils::fastest_axis (sparse.rs:400-406)
+    }
+
+    /// CsMat::to_dense (csmat.rs:1127-1134): C order, stored values as bits, +0.0 elsewhere.
+    pub fn to_dense<I: SpIndex, Iptr: SpIndex>(m: &DeviceCsMat<I, Iptr>) -> Array2<f64> {
+        let (r, c) = (m.host.rows(), m.host.cols());
+        let mut out = Array2::<f64>::zeros((r, c));
+        if r > 0 && c > 0 {
+            CTX.with(|x| check(x.0, unsafe {
+                ffi::sprs_b200_csmat_to_dense(x.0, m.dev, out.as_mut_ptr(), c as u64) }))
+                .expect("sprs_b200 device error");
+        }
+        out
+    }
+
+    /// assign_to_dense (to_dense.rs:12-30): every stored value into `array`, the rest untouched.
+    pub fn assign_to_dense<I: SpIndex, Iptr: SpIndex>(mut array: ArrayViewMut2<f64>, m: &DeviceCsMat<I, Iptr>) {
+        assert_eq!(m.host.cols(), array.shape()[1], "Dimension mismatch");
+        assert_eq!(m.host.rows(), array.shape()[0], "Dimension mismatch");
+        let (rs, cs) = strides(&array);
+        let (r, c) = (array.shape()[0] as u64, array.shape()[1] as u64);
+        CTX.with(|x| check(x.0, unsafe {
+            ffi::sprs_b200_assign_to_dense(x.0, m.dev, array.as_mut_ptr(), r, c, rs, cs) }))
+            .expect("sprs_b200 device error");
+    }
+
+    fn from_dense<S: Data<Elem = f64>, I: SpIndex, Iptr: SpIndex>(m: &ArrayBase<S, Ix2>, epsilon: f64, csr: bool) -> CsMatI<f64, I, Iptr> {
+        let (rs, cs) = strides(m);
+        let (r, c) = (m.shape()[0], m.shape()[1]);
+        let st = if csr { ffi::SPRS_B200_CSR } else { ffi::SPRS_B200_CSC };
+        CTX.with(|x| {
+            let mut out = std::ptr::null_mut();
+            check(x.0, unsafe { ffi::sprs_b200_csmat_from_dense(x.0, st, r as u64, c as u64, m.as_ptr(),
+                                                                rs, cs, epsilon, &mut out) })
+                .expect("sprs_b200 device error");
+            let like: CsMatI<f64, I, Iptr> = if csr { CsMatI::zero((r, c)) } else { CsMatI::zero((r, c)).to_csc() };
+            download_result(x.0, out, &like)
+        })
+    }
+    /// CsMat::csr_from_dense (csmat.rs:502-539): |x| > epsilon kept (epsilon clamped to +0.0
+    /// unless > 0), values as bits, columns ascending in each row.
+    pub fn csr_from_dense<S: Data<Elem = f64>, I: SpIndex, Iptr: SpIndex>(m: &ArrayBase<S, Ix2>, epsilon: f64) -> CsMatI<f64, I, Iptr> {
+        from_dense(m, epsilon, true)
+    }
+    /// CsMat::csc_from_dense (csmat.rs:544-549).
+    pub fn csc_from_dense<S: Data<Elem = f64>, I: SpIndex, Iptr: SpIndex>(m: &ArrayBase<S, Ix2>, epsilon: f64) -> CsMatI<f64, I, Iptr> {
+        from_dense(m, epsilon, false)
+    }
+
+    fn binop_dense<S: Data<Elem = f64>, I: SpIndex, Iptr: SpIndex>(lhs: *const ffi::sprs_b200_csmat, op: i32, alpha: f64,
+                                                                   beta: f64, rhs: &ArrayBase<S, Ix2>) -> Array2<f64> {
+        let shape = (rhs.shape()[0], rhs.shape()[1]);
+        let mut out = if c_like(rhs) { Array2::zeros(shape) } else { Array2::zeros(shape.f()) };
+        let (rrs, rcs) = strides(rhs);
+        let (ors, ocs) = strides(&out);
+        CTX.with(|x| check(x.0, unsafe {
+            ffi::sprs_b200_csmat_binop_dense(x.0, lhs, op, alpha, beta, rhs.as_ptr(), shape.0 as u64,
+                                             shape.1 as u64, rrs, rcs, out.as_mut_ptr(), shape.0 as u64,
+                                             shape.1 as u64, ors, ocs) }))
+            .expect("sprs_b200 device error");
+        out
+    }
+    /// binop::add_dense_mat_same_ordering (binop.rs:279-323): (alpha*x) + (beta*y).
+    pub fn add_dense_mat_same_ordering<S: Data<Elem = f64>, I: SpIndex, Iptr: SpIndex>(
+        lhs: &DeviceCsMat<I, Iptr>, rhs: &ArrayBase<S, Ix2>, alpha: f64, beta: f64) -> Array2<f64> {
+        binop_dense::<S, I, Iptr>(lhs.dev, ffi::SPRS_B200_BINOP_ADD, alpha, beta, rhs)
+    }
+    /// binop::mul_dense_mat_same_ordering (binop.rs:331-371): (alpha*x)*y.
+    pub fn mul_dense_mat_same_ordering<S: Data<Elem = f64>, I: SpIndex, Iptr: SpIndex>(
+        lhs: &DeviceCsMat<I, Iptr>, rhs: &ArrayBase<S, Ix2>, alpha: f64) -> Array2<f64> {
+        binop_dense::<S, I, Iptr>(lhs.dev, ffi::SPRS_B200_BINOP_MUL, alpha, 0.0, rhs)
+    }
+    /// `&A + &D` (csmat.rs:1951-1987): A converted first when its storage does not match D's
+    /// fastest axis; the result has D's layout.
+    pub fn add_dense<S: Data<Elem = f64>, I: SpIndex, Iptr: SpIndex>(a: &DeviceCsMat<I, Iptr>, d: &ArrayBase<S, Ix2>) -> Array2<f64> {
+        if a.host.is_csr() == c_like(d) { return add_dense_mat_same_ordering(a, d, 1.0, 1.0); }
+        CTX.with(|x| {
+            let mut conv = std::ptr::null_mut();
+            check(x.0, unsafe { ffi::sprs_b200_csmat_to_other_storage(x.0, a.dev, &mut conv) })
+                .expect("sprs_b200 device error");
+            let out = binop_dense::<S, I, Iptr>(conv, ffi::SPRS_B200_BINOP_ADD, 1.0, 1.0, d);
+            unsafe { ffi::sprs_b200_csmat_free(conv); }
+            out
+        })
+    }
+}
+
 /// sprs::bmat / vstack / hstack (construct.rs) and sprs::kronecker_product (kronecker.rs) on the
 /// device, bit-identical to the reference (csrc/construct.cu).  The asserts run here in the
 /// reference's order; a result dimension >= 2^32 is a device error (u32 mirrors) even where

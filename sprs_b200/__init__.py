@@ -9,13 +9,15 @@ from . import _lib, construct, io, ldl, linalg
 from .construct import bmat, hstack, kronecker_product, vstack
 from .ldl import is_symmetric
 from .sparse import (CSC, CSR, Context, CsMat, CsVec, DeviceCsMat, SingularMatrix, SprsPanic,
-                     ThirdPartyError, binop, csmat_mul_csmat, prod, smmp)
+                     ThirdPartyError, assign_to_dense, binop, csmat_mul_csmat, prod, smmp)
 
 __all__ = ["CSC", "CSR", "Context", "CsMat", "CsVec", "DeviceCsMat", "SingularMatrix", "SprsPanic",
-           "ThirdPartyError", "binop", "bmat", "construct", "csmat_mul_csmat", "hstack",
+           "ThirdPartyError", "assign_to_dense", "binop", "bmat", "construct", "csmat_mul_csmat", "hstack",
            "is_symmetric", "kronecker_product", "prod", "smmp", "vstack", "_lib", "io", "ldl",
            "linalg"]
 CONSTRUCT_TILE = 2048  # output entries per warp tile of the construction kernels (csrc/construct.cu)
+DENSE_TILE = 4096      # positions per warp tile of the dense-boundary kernels (csrc/transpose.cu)
+SCATTER_TILE = 256     # stored entries per warp tile of assign_to_dense (csrc/transpose.cu)
 __version__ = "0.1.0"
 import os as _os
 

@@ -54,6 +54,17 @@ PROTOTYPES = {
     "sprs_b200_csmat_bmat": (_int, [_vp, _u64, _u64, C.POINTER(_vp), C.POINTER(_vp)]),
     "sprs_b200_csmat_kron": (_int, [_vp, _vp, _vp, C.POINTER(_vp)]),
     "sprs_b200_csmat_transpose_view": (_int, [_vp, _vp, C.POINTER(_vp)]),
+    "sprs_b200_csmat_to_dense": (_int, [_vp, _vp, _dp, _u64]),
+    "sprs_b200_csmat_to_dense_dev": (_int, [_vp, _vp, _dp, _u64, _vp]),
+    "sprs_b200_assign_to_dense": (_int, [_vp, _vp, _dp, _u64, _u64, _i64, _i64]),
+    "sprs_b200_assign_to_dense_dev": (_int, [_vp, _vp, _dp, _u64, _u64, _i64, _i64, _vp]),
+    "sprs_b200_csmat_from_dense": (_int, [_vp, _int, _u64, _u64, _dp, _i64, _i64, C.c_double,
+                                          C.POINTER(_vp)]),
+    "sprs_b200_csmat_from_dense_dev": (_int, [_vp, _int, _u64, _u64, _dp, _i64, _i64, C.c_double,
+                                              C.POINTER(_vp)]),
+    "sprs_b200_csmat_binop_dense": (_int, [_vp, _vp, _int, C.c_double, C.c_double] + _dense_sig[2:]),
+    "sprs_b200_csmat_binop_dense_dev": (_int, [_vp, _vp, _int, C.c_double, C.c_double] +
+                                        _dense_sig[2:] + [_vp]),
     "sprs_b200_mul_acc_mat_vec_csr": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
     "sprs_b200_mul_acc_mat_vec_csc": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),
     "sprs_b200_mul_mat_vec": (_int, [_vp, _vp, _dp, _u64, _dp, _u64]),

@@ -845,6 +845,55 @@ int sprs_b200_csc_mulacc_dense_colmaj(sprs_b200_ctx* ctx, const sprs_b200_csmat*
 
 }  // extern "C"
 
+// ---- device-built results (declared in common.cuh): the binops, scale, construct.cu and
+// the dense boundary in transpose.cu build their result mirrors with these
+bool force_indptr64() {
+    // the SPRS_B200_FORCE_INDPTR64 test hook of csmat_upload, applied to the results too
+    static const bool force64 = [] {
+        const char* v = getenv("SPRS_B200_FORCE_INDPTR64");
+        return v && atoi(v) != 0;
+    }();
+    return force64;
+}
+
+sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
+                            uint64_t nnz, int indptr_bytes) {
+    auto* m = new sprs_b200_csmat();
+    m->ctx = ctx;
+    m->storage = storage;
+    m->rows = rows;
+    m->cols = cols;
+    m->outer = storage == SPRS_B200_CSR ? rows : cols;
+    m->inner = storage == SPRS_B200_CSR ? cols : rows;
+    m->nnz = nnz;
+    m->indptr_bytes = indptr_bytes;
+    m->pooled = true;
+    return m;
+}
+
+sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, const sprs_b200_csmat* like, uint64_t nnz,
+                            int indptr_bytes) {
+    return new_result(ctx, like->storage, like->rows, like->cols, nnz, indptr_bytes);
+}
+
+int alloc_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s) {
+    if (cudaMallocAsync(&m->d_indptr, (m->outer + 1) * (size_t)m->indptr_bytes + 16, s) != cudaSuccess ||
+        cudaMallocAsync((void**)&m->d_indices, m->nnz * 4 + 16, s) != cudaSuccess ||
+        cudaMallocAsync((void**)&m->d_data, m->nnz * 8 + 16, s) != cudaSuccess) {
+        cudaGetLastError();
+        SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "binop: cudaMallocAsync of the result failed");
+    }
+    return SPRS_B200_OK;
+}
+
+// The result's SpMV partition (no hot set: its build would run inside every call), then wait.
+int finish_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, const char* what) {
+    SPRS_TRY(spmv_prepare(ctx, m, s, false));
+    if (cudaStreamSynchronize(s) != cudaSuccess || cudaGetLastError() != cudaSuccess)
+        SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "%s: kernel failed", what);
+    return SPRS_B200_OK;
+}
+
 int csmat_csr_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const sprs_b200_csmat** out) {
     return csr_of(ctx, m, out);
 }

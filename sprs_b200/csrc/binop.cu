@@ -225,53 +225,6 @@ __global__ void scale_kernel(const P* __restrict__ ip, const uint32_t* __restric
         ip_out[i] = ip[i];
 }
 
-}  // namespace
-
-// ---- result helpers, shared with construct.cu (declared in common.cuh)
-bool force_indptr64() {
-    // the SPRS_B200_FORCE_INDPTR64 test hook of csmat_upload, applied to the results too
-    static const bool force64 = [] {
-        const char* v = getenv("SPRS_B200_FORCE_INDPTR64");
-        return v && atoi(v) != 0;
-    }();
-    return force64;
-}
-
-sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, const sprs_b200_csmat* like, uint64_t nnz,
-                            int indptr_bytes) {
-    auto* m = new sprs_b200_csmat();
-    m->ctx = ctx;
-    m->storage = like->storage;
-    m->rows = like->rows;
-    m->cols = like->cols;
-    m->outer = like->outer;
-    m->inner = like->inner;
-    m->nnz = nnz;
-    m->indptr_bytes = indptr_bytes;
-    m->pooled = true;
-    return m;
-}
-
-int alloc_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s) {
-    if (cudaMallocAsync(&m->d_indptr, (m->outer + 1) * (size_t)m->indptr_bytes + 16, s) != cudaSuccess ||
-        cudaMallocAsync((void**)&m->d_indices, m->nnz * 4 + 16, s) != cudaSuccess ||
-        cudaMallocAsync((void**)&m->d_data, m->nnz * 8 + 16, s) != cudaSuccess) {
-        cudaGetLastError();
-        SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "binop: cudaMallocAsync of the result failed");
-    }
-    return SPRS_B200_OK;
-}
-
-// The result's SpMV partition (no hot set: its build would run inside every call), then wait.
-int finish_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, const char* what) {
-    SPRS_TRY(spmv_prepare(ctx, m, s, false));
-    if (cudaStreamSynchronize(s) != cudaSuccess || cudaGetLastError() != cudaSuccess)
-        SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "%s: kernel failed", what);
-    return SPRS_B200_OK;
-}
-
-namespace {
-
 template <typename PA, typename PB, typename PC>
 void launch_fill(const Operands<PA, PB>& o, int op, uint64_t total, uint64_t n_tiles,
                  const uint32_t* cut_r, const uint64_t* cut_a, const uint64_t* cut_b,

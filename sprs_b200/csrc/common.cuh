@@ -151,12 +151,15 @@ int transpose_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, sprs_b200_csm
 // device conversion, owned by the mirror (api.cu)
 int csmat_csr_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const sprs_b200_csmat** out);
 
-// ---- device-built results (binop.cu; the binops, scale and construct.cu use them)
+// ---- device-built results (api.cu; the binops, scale, construct.cu and the dense boundary in transpose.cu use them)
 // the SPRS_B200_FORCE_INDPTR64 test hook of csmat_upload, applied to the results too
 bool force_indptr64();
 // a pooled result mirror with like's storage and shape (no arrays yet)
 sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, const sprs_b200_csmat* like, uint64_t nnz,
                             int indptr_bytes);
+// the same with the storage and shape given
+sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
+                            uint64_t nnz, int indptr_bytes);
 // its indptr / indices / data, stream-ordered on s
 int alloc_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s);
 // its SpMV partition (no hot set), then wait for s

@@ -345,3 +345,67 @@ def kron(ctx, a, b):
     if _device(ctx).type == "cuda":
         _sync()
     return _with_views(ctx, kron_dev(ctx, ma, mb))
+
+
+# ---- the dense boundary on torch tensors (the dense section of csrc/transpose.cu)
+def _strides(t):
+    """element strides of a 2-D float64 tensor as the library takes them (all zero for a tensor
+    with a zero-length axis, as ndarray has them)"""
+    if t.dim() != 2 or t.dtype != torch.float64:
+        raise TypeError("a 2-D float64 tensor is required")
+    return (0, 0) if 0 in t.shape else (t.stride(0), t.stride(1))
+
+
+def to_dense(ctx, a, out=None):
+    """CsMat::to_dense (csmat.rs:1127-1134) on the device: a C-order tensor (out, if given, must
+    have unit column stride) holding A's values as bits and +0.0 elsewhere; torch's stream."""
+    m = a.mirror if isinstance(a, DeviceCsr) else a
+    if out is None:
+        out = torch.empty((m.rows, m.cols), dtype=torch.float64, device=_device(ctx))
+    if out.shape != (m.rows, m.cols) or (out.numel() and out.stride(1) != 1):
+        raise ValueError("out must be a (rows, cols) tensor with unit column stride")
+    ld = out.stride(0) if out.numel() else m.cols
+    ctx.check(ctx.lib.sprs_b200_csmat_to_dense_dev(ctx.h, m.h, _dptr(out), ld, _stream_ptr()))
+    return out
+
+
+def assign_to_dense(ctx, out, a):
+    """assign_to_dense (to_dense.rs:12-30) into a 2-D float64 tensor view: A's values as bits,
+    every other element untouched; torch's stream."""
+    m = a.mirror if isinstance(a, DeviceCsr) else a
+    rs, cs = _strides(out)
+    ctx.check(ctx.lib.sprs_b200_assign_to_dense_dev(ctx.h, m.h, _dptr(out), out.shape[0],
+                                                    out.shape[1], rs, cs, _stream_ptr()))
+    return out
+
+
+def from_dense(ctx, d, epsilon, storage="CSR"):
+    """csr_from_dense / csc_from_dense (csmat.rs:502-549) of a 2-D float64 tensor view.  Returns
+    (mirror, indptr, indices, data) like binop: the DeviceCsMat that owns the result and
+    zero-copy torch views of its arrays."""
+    rs, cs = _strides(d)
+    if _device(ctx).type == "cuda":
+        _sync()  # d produced on torch's stream; the passes run on the ctx stream
+    cm = C.c_void_p()
+    ctx.check(ctx.lib.sprs_b200_csmat_from_dense_dev(
+        ctx.h, _lib.CSR if storage == "CSR" else _lib.CSC, d.shape[0], d.shape[1], _dptr(d), rs, cs,
+        float(epsilon), C.byref(cm)))
+    return _with_views(ctx, DeviceCsMat(ctx, cm))
+
+
+def binop_dense(ctx, a, d, op="add", alpha=1.0, beta=1.0, out=None):
+    """csmat_binop_dense_raw (binop.rs:384-433) on the device: out = alpha*A + beta*D ("add") or
+    alpha*A*D ("mul"), A's storage matching the fastest axis of D and out.  out=None allocates it
+    as add_dense_mat_same_ordering does (C order when D's fastest axis is Axis(1), F order
+    otherwise); out may be d itself.  torch's stream."""
+    m = a.mirror if isinstance(a, DeviceCsr) else a
+    rrs, rcs = _strides(d)
+    if out is None:
+        out = torch.empty(d.shape, dtype=torch.float64, device=_device(ctx))
+        if rcs > rrs:  # Axis(0) fastest: F order
+            out = torch.empty((d.shape[1], d.shape[0]), dtype=torch.float64, device=_device(ctx)).t()
+    ors, ocs = _strides(out)
+    ctx.check(ctx.lib.sprs_b200_csmat_binop_dense_dev(
+        ctx.h, m.h, _BINOP_OPS[op], float(alpha), float(beta), _dptr(d), d.shape[0], d.shape[1], rrs,
+        rcs, _dptr(out), out.shape[0], out.shape[1], ors, ocs, _stream_ptr()))
+    return out

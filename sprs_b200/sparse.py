@@ -12,6 +12,9 @@ reference's own tests.  Same names, argument meaning and error behaviour:
   smmp.mul_csr_csr, symbolic+numeric  sprs/src/sparse/smmp.rs
   a + b, a - b, a * s                 `impl Add/Sub/Mul<N>` sprs/src/sparse/binop.rs:20-163
   binop.mul_mat_same_storage          sprs/src/sparse/binop.rs:115-130
+  to_dense, assign_to_dense           sprs/src/sparse/csmat.rs:1127-1134, to_dense.rs:12-30
+  csr_from_dense / csc_from_dense     sprs/src/sparse/csmat.rs:502-549
+  a + D, binop.{add,mul}_dense_...    csmat.rs:1951-1987, binop.rs:273-433
 
 Contract violations raise SprsPanic with the reference's panic message
 ("Dimension mismatch", "Storage mismatch"; sprs Guidelines.rst:9-27); device
@@ -410,15 +413,27 @@ class CsMat:
         return t
 
     def to_dense(self):
-        out = np.zeros(self.shape)
-        ip = self.indptr.astype(np.int64) - int(self.indptr[0])
-        for o in range(self.outer_dims()):
-            for k in range(ip[o], ip[o + 1]):
-                if self.storage == CSR:
-                    out[o, self.indices[k]] = self.data[k]
-                else:
-                    out[self.indices[k], o] = self.data[k]
+        """CsMat::to_dense (csmat.rs:1127-1134) on the device: a C-order array holding every
+        stored value as its exact bits and +0.0 everywhere else, for CSR and CSC alike."""
+        out = np.empty(self.shape)  # the device writes every element
+        if out.size:
+            ctx = self.context()
+            ctx.check(ctx.lib.sprs_b200_csmat_to_dense(ctx.h, self.device().h, _ptr(out),
+                                                       self.shape[1]))
         return out
+
+    @classmethod
+    def csr_from_dense(cls, m, epsilon, index_dtype=np.uint64, ctx=None):
+        """CsMat::csr_from_dense (csmat.rs:502-539) on the device: every x of the 2-D float64
+        view m with |x| > epsilon, epsilon clamped to +0.0 when it is not > 0 (so +-0.0 and NaN
+        are never kept), stored as the same bits, columns ascending within each row."""
+        return _from_dense(cls, m, epsilon, CSR, index_dtype, ctx)
+
+    @classmethod
+    def csc_from_dense(cls, m, epsilon, index_dtype=np.uint64, ctx=None):
+        """CsMat::csc_from_dense (csmat.rs:544-549): csr_from_dense of the transposed view,
+        transposed -- a CSC matrix with rows ascending within each column."""
+        return _from_dense(cls, m, epsilon, CSC, index_dtype, ctx)
 
     # -- device mirror
     def context(self):
@@ -483,6 +498,8 @@ class CsMat:
         to_other_storage when the storages differ; entries whose sum is 0.0 are dropped."""
         if isinstance(rhs, CsMat):
             return _csmat_binop_other_storage(self, rhs, _lib.BINOP_ADD)
+        if isinstance(rhs, np.ndarray) and rhs.ndim == 2:
+            return _csmat_add_dense(self, rhs)
         return NotImplemented
 
     def __sub__(self, rhs):
@@ -547,6 +564,115 @@ class binop:
         if lhs.storage != rhs.storage:
             raise SprsPanic("Storage mismatch")
         return _csmat_binop(lhs, rhs.device(), _lib.BINOP_MUL)
+
+    @staticmethod
+    def add_dense_mat_same_ordering(lhs, rhs, alpha, beta):
+        """binop.rs:279-323: alpha * lhs + beta * rhs, lhs sparse, rhs a 2-D float64 view, as
+        (alpha*x) + (beta*y) with x = +0.0 where lhs has no entry.  The result is C order when
+        rhs's fastest axis is Axis(1), F order otherwise; a CSR lhs needs a C-like rhs and a CSC
+        one an F-like rhs ("Storage mismatch"), after the shapes ("Dimension mismatch")."""
+        out = np.zeros(rhs.shape, order="C" if fastest_axis(rhs) == 1 else "F")
+        _binop_dense(lhs.device(), _lib.BINOP_ADD, alpha, beta, rhs, out)
+        return out
+
+    @staticmethod
+    def mul_dense_mat_same_ordering(lhs, rhs, alpha):
+        """binop.rs:331-371: (alpha*x)*y element-wise, x = +0.0 where lhs has no entry, so a
+        missing position gives -0.0 for a negative y and NaN for an infinite or NaN y.  Layout
+        and panics as add_dense_mat_same_ordering."""
+        out = np.zeros(rhs.shape, order="C" if fastest_axis(rhs) == 1 else "F")
+        _binop_dense(lhs.device(), _lib.BINOP_MUL, alpha, 0.0, rhs, out)
+        return out
+
+    @staticmethod
+    def csmat_binop_dense_raw_add(lhs, rhs, alpha, beta, out):
+        """csmat_binop_dense_raw (binop.rs:384-433) with the add closure, into the given writeable
+        out view (which may be rhs itself)."""
+        _binop_dense(lhs.device(), _lib.BINOP_ADD, alpha, beta, rhs, out)
+
+    @staticmethod
+    def csmat_binop_dense_raw_mul(lhs, rhs, alpha, out):
+        """csmat_binop_dense_raw with the mul closure, into out."""
+        _binop_dense(lhs.device(), _lib.BINOP_MUL, alpha, 0.0, rhs, out)
+
+
+# ---- the dense boundary: to_dense.rs, csmat.rs:502-549, binop.rs:273-433
+def dense_strides(a, writeable=False):
+    """The element strides (rs, cs) a float64 2-D view is passed to the library with.  ndarray
+    gives an array with a zero-length axis all-zero strides (its default C and F strides and
+    its slicing both do), where numpy keeps non-zero ones: such a view is passed as (0, 0), so
+    that fastest_axis sees what the reference sees (DESIGN.md 4.11)."""
+    if not isinstance(a, np.ndarray) or a.ndim != 2:
+        raise TypeError("a 2-D numpy array is required (ArrayView2)")
+    if a.dtype != np.float64:
+        raise TypeError("f64 only on the H100 path (other N stay on the CPU code)")
+    if writeable and not a.flags.writeable:
+        raise ValueError("the dense array must be writeable (ArrayViewMut)")
+    if 0 in a.shape:
+        return 0, 0
+    if a.strides[0] % 8 or a.strides[1] % 8:
+        raise TypeError("strides must be whole float64 elements")
+    return a.strides[0] // 8, a.strides[1] // 8
+
+
+def fastest_axis(a):
+    """utils::fastest_axis (sparse.rs:400-406): Axis(0) iff strides[1] > strides[0] (signed);
+    equal strides -- length-1 axes, broadcasts, empty arrays -- give Axis(1)."""
+    rs, cs = dense_strides(a)
+    return 0 if cs > rs else 1
+
+
+def assign_to_dense(array, spmat):
+    """to_dense.rs:12-30: array[r, c] = v for every stored (v, (r, c)) of spmat, copied as bits;
+    every other element of the writeable view is left as it is.  Asserts cols, then rows."""
+    rs, cs = dense_strides(array, writeable=True)
+    if spmat.cols() != array.shape[1] or spmat.rows() != array.shape[0]:
+        raise SprsPanic("Dimension mismatch")
+    ctx = spmat.context()
+    ctx.check(ctx.lib.sprs_b200_assign_to_dense(ctx.h, spmat.device().h, _ptr(array),
+                                                array.shape[0], array.shape[1], rs, cs))
+
+
+def _binop_dense(lhs_dev, op, alpha, beta, rhs, out):
+    """csmat_binop_dense_raw on the device: shapes, then storage, checked by the library in the
+    reference's order."""
+    rrs, rcs = dense_strides(rhs)
+    ors, ocs = dense_strides(out, writeable=True)
+    ctx = lhs_dev.ctx
+    ctx.check(ctx.lib.sprs_b200_csmat_binop_dense(
+        ctx.h, lhs_dev.h, op, float(alpha), float(beta), _ptr(rhs), rhs.shape[0], rhs.shape[1],
+        rrs, rcs, _ptr(out), out.shape[0], out.shape[1], ors, ocs))
+
+
+def _csmat_add_dense(a, d):
+    """`&A + &D` (csmat.rs:1951-1987): alpha = beta = 1; A converted with to_other_storage first
+    when its storage does not match D's fastest axis; the result has D's layout."""
+    c_like = fastest_axis(d) == 1
+    lhs = a.device() if a.is_csr() == c_like else a.device().to_other_storage()
+    out = np.zeros(d.shape, order="C" if c_like else "F")
+    _binop_dense(lhs, _lib.BINOP_ADD, 1.0, 1.0, d, out)
+    return out
+
+
+def _from_dense(cls, m, epsilon, storage, index_dtype, ctx):
+    rs, cs = dense_strides(m)
+    ctx = ctx or Context.default()
+    h = C.c_void_p()
+    ctx.check(ctx.lib.sprs_b200_csmat_from_dense(ctx.h, _STOR[storage], m.shape[0], m.shape[1],
+                                                 _ptr(m), rs, cs, float(epsilon), C.byref(h)))
+    dev = DeviceCsMat(ctx, h)
+    ip, ind, dat = dev.download(np.uint64)
+    # Iptr::from_usize / I::from_usize (indexing.rs:104-107): the indptr is built first
+    mx = np.iinfo(index_dtype).max
+    for a in (ip, ind):
+        big = np.nonzero(a > mx)[0]
+        if big.size:
+            raise SprsPanic("Failed to convert %d to index type" % int(a[big[0]]))
+    out = object.__new__(cls)
+    out.storage, out.shape = storage, (int(m.shape[0]), int(m.shape[1]))
+    out.indptr, out.indices, out.data = ip.astype(index_dtype), ind.astype(index_dtype), dat
+    out._ctx, out._dev = ctx, dev
+    return out
 
 
 # `impl Mul<&ArrayBase<_, Ix1>> for &CsMatBase`  csmat.rs:2119-2160
