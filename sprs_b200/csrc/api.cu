@@ -312,60 +312,16 @@ int sprs_b200_csmat_upload(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint6
     const uint64_t nnz = last - base;
     if (nnz > 0 && (!indices || !data)) return SPRS_B200_ERR_ARGUMENT;
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
-
-    auto* m = new sprs_b200_csmat();
-    m->ctx = ctx;
-    m->storage = storage;
-    m->rows = rows;
-    m->cols = cols;
-    m->nnz = nnz;
-    m->outer = outer;
-    m->inner = storage == SPRS_B200_CSR ? cols : rows;
-    // 64-bit indptr only when nnz needs it; SPRS_B200_FORCE_INDPTR64=1 is a TEST hook that
-    // takes the uint64 instantiations of the kernels at sizes a test can afford
-    static const bool force64 = [] {
-        const char* v = getenv("SPRS_B200_FORCE_INDPTR64");
-        return v && atoi(v) != 0;
-    }();
-    m->indptr_bytes = (nnz >= 0xffffffffull || force64) ? 8 : 4;
+    CsmatPtr m = new_result(ctx, storage, rows, cols, nnz, indptr_bytes_for(nnz), Arrays::owned);
     cudaStream_t s = ctx->stream;
-    int st = SPRS_B200_OK;
-    do {
-        cudaError_t e;
-        if ((e = cudaMalloc(&m->d_indptr, (outer + 1) * (size_t)m->indptr_bytes + 16)) != cudaSuccess ||
-            (e = cudaMalloc((void**)&m->d_indices, nnz * sizeof(uint32_t) + 16)) != cudaSuccess ||
-            (e = cudaMalloc((void**)&m->d_data, nnz * sizeof(double) + 16)) != cudaSuccess) {
-            sprs_b200_set_error(ctx, (std::string("cudaMalloc: ") + cudaGetErrorString(e)).c_str());
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        if ((st = upload_indexlike(ctx, indptr, indptr_bytes, outer + 1, base, m->d_indptr,
-                                   m->indptr_bytes, s)) != SPRS_B200_OK)
-            break;
-        if ((st = upload_indexlike(ctx, indices, index_bytes, nnz, 0, m->d_indices, 4, s)) !=
-            SPRS_B200_OK)
-            break;
-        if (nnz > 0) {
-            e = cudaMemcpyAsync(m->d_data, data, nnz * sizeof(double), cudaMemcpyHostToDevice, s);
-            if (e != cudaSuccess) {
-                sprs_b200_set_error(ctx, cudaGetErrorString(e));
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-        }
-        if ((st = spmv_prepare(ctx, m, s)) != SPRS_B200_OK) break;
-        e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) {
-            sprs_b200_set_error(ctx, cudaGetErrorString(e));
-            st = SPRS_B200_ERR_CUDA;
-        }
-    } while (0);
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(m);
-        return st;
-    }
-    *out = m;
-    return SPRS_B200_OK;
+    SPRS_TRY(alloc_result(ctx, m.get(), s, "upload"));
+    SPRS_TRY(upload_indexlike(ctx, indptr, indptr_bytes, outer + 1, base, m->d_indptr,
+                              m->indptr_bytes, s));
+    SPRS_TRY(upload_indexlike(ctx, indices, index_bytes, nnz, 0, m->d_indices, 4, s));
+    if (nnz > 0)
+        SPRS_CUDA(ctx, cudaMemcpyAsync(m->d_data, data, nnz * sizeof(double),
+                                       cudaMemcpyHostToDevice, s));
+    return finish_result(ctx, m, s, "upload", true, out);
 }
 
 int sprs_b200_csmat_from_device(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
@@ -379,30 +335,11 @@ int sprs_b200_csmat_from_device(sprs_b200_ctx* ctx, int storage, uint64_t rows, 
     if (((uintptr_t)d_indices | (uintptr_t)d_data) & 15)
         SPRS_FAIL(ctx, SPRS_B200_ERR_ARGUMENT, "device arrays must be 16-byte aligned");
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
-    auto* m = new sprs_b200_csmat();
-    m->ctx = ctx;
-    m->storage = storage;
-    m->rows = rows;
-    m->cols = cols;
-    m->nnz = nnz;
-    m->outer = storage == SPRS_B200_CSR ? rows : cols;
-    m->inner = storage == SPRS_B200_CSR ? cols : rows;
-    m->indptr_bytes = 4;
+    CsmatPtr m = new_result(ctx, storage, rows, cols, nnz, 4, Arrays::borrowed);
     m->d_indptr = const_cast<uint32_t*>(d_indptr);
     m->d_indices = const_cast<uint32_t*>(d_indices);
     m->d_data = const_cast<double*>(d_data);
-    m->owns = false;
-    int st = spmv_prepare(ctx, m, ctx->stream);
-    if (st == SPRS_B200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-        sprs_b200_set_error(ctx, "from_device: partition kernel failed");
-        st = SPRS_B200_ERR_CUDA;
-    }
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(m);
-        return st;
-    }
-    *out = m;
-    return SPRS_B200_OK;
+    return finish_result(ctx, m, ctx->stream, "from_device", true, out);
 }
 
 int sprs_b200_csmat_free(sprs_b200_csmat* m) {
@@ -425,22 +362,6 @@ int sprs_b200_csmat_free(sprs_b200_csmat* m) {
     if (m->d_hot_idx) cudaFree(m->d_hot_idx);
     if (m->csr_cache) sprs_b200_csmat_free(m->csr_cache);
     delete m;
-    return SPRS_B200_OK;
-}
-
-// CSR view of a mirror for the product kernels: the mirror itself, or (CSC) its cached
-// device conversion -- same sums in the same order (ascending column per output element).
-static int csr_of(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const sprs_b200_csmat** out) {
-    if (m->storage == SPRS_B200_CSR) {
-        *out = m;
-        return SPRS_B200_OK;
-    }
-    if (!m->csr_cache) {
-        sprs_b200_csmat* t = nullptr;
-        SPRS_TRY(sprs_b200_csmat_to_other_storage(ctx, m, &t));
-        m->csr_cache = t;
-    }
-    *out = m->csr_cache;
     return SPRS_B200_OK;
 }
 
@@ -481,29 +402,15 @@ int sprs_b200_csmat_device_arrays(const sprs_b200_csmat* m, const void** d_indpt
     return SPRS_B200_OK;
 }
 
-static int finish_triplets(sprs_b200_ctx* ctx, sprs_b200_csmat* t, int st, sprs_b200_csmat** out) {
-    if (st == SPRS_B200_OK) st = spmv_prepare(ctx, t, ctx->stream);
-    if (st == SPRS_B200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-        sprs_b200_set_error(ctx, "from_triplets: kernel failed");
-        st = SPRS_B200_ERR_CUDA;
-    }
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(t);
-        return st;
-    }
-    *out = t;
-    return SPRS_B200_OK;
-}
-
 int sprs_b200_csmat_from_triplets_dev(sprs_b200_ctx* ctx, uint64_t rows, uint64_t cols,
                                       uint64_t n, const uint32_t* d_row, const uint32_t* d_col,
                                       const double* d_val, sprs_b200_csmat** out) {
     if (!ctx || !out || (n && (!d_row || !d_col || !d_val))) return SPRS_B200_ERR_ARGUMENT;
     *out = nullptr;
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
-    auto* t = new sprs_b200_csmat();
-    return finish_triplets(ctx, t, triplets_to_csr_launch(ctx, rows, cols, n, d_row, d_col, d_val,
-                                                         t, ctx->stream), out);
+    CsmatPtr t;
+    SPRS_TRY(triplets_to_csr_launch(ctx, rows, cols, n, d_row, d_col, d_val, &t, ctx->stream));
+    return finish_result(ctx, t, ctx->stream, "from_triplets", true, out);
 }
 
 int sprs_b200_csmat_from_triplets(sprs_b200_ctx* ctx, uint64_t rows, uint64_t cols, uint64_t n,
@@ -517,31 +424,19 @@ int sprs_b200_csmat_from_triplets(sprs_b200_ctx* ctx, uint64_t rows, uint64_t co
         SPRS_FAIL(ctx, SPRS_B200_ERR_INDEX_RANGE, "from_triplets: needs nnz, rows, cols < 2^32");
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
-    uint32_t *d_row = nullptr, *d_col = nullptr;
-    double* d_val = nullptr;
-    int st = SPRS_B200_OK;
-    auto* t = new sprs_b200_csmat();
-    do {
-        if (cudaMalloc((void**)&d_row, n * 4 + 16) != cudaSuccess ||
-            cudaMalloc((void**)&d_col, n * 4 + 16) != cudaSuccess ||
-            cudaMalloc((void**)&d_val, n * 8 + 16) != cudaSuccess) {
-            sprs_b200_set_error(ctx, "from_triplets: cudaMalloc failed");
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        if ((st = upload_indexlike(ctx, row_inds, index_bytes, n, 0, d_row, 4, s)) != SPRS_B200_OK) break;
-        if ((st = upload_indexlike(ctx, col_inds, index_bytes, n, 0, d_col, 4, s)) != SPRS_B200_OK) break;
-        if (n && cudaMemcpyAsync(d_val, data, n * 8, cudaMemcpyHostToDevice, s) != cudaSuccess) {
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        st = triplets_to_csr_launch(ctx, rows, cols, n, d_row, d_col, d_val, t, s);
-    } while (0);
-    cudaStreamSynchronize(s);
-    if (d_row) cudaFree(d_row);
-    if (d_col) cudaFree(d_col);
-    if (d_val) cudaFree(d_val);
-    return finish_triplets(ctx, t, st, out);
+    CsmatPtr t;
+    {   // the device copies of the triplets live until the CSR mirror is built
+        Owned<uint32_t> d_row, d_col;
+        Owned<double> d_val;
+        SPRS_TRY(d_row.alloc(ctx, n * 4 + 16, "from_triplets"));
+        SPRS_TRY(d_col.alloc(ctx, n * 4 + 16, "from_triplets"));
+        SPRS_TRY(d_val.alloc(ctx, n * 8 + 16, "from_triplets"));
+        SPRS_TRY(upload_indexlike(ctx, row_inds, index_bytes, n, 0, d_row, 4, s));
+        SPRS_TRY(upload_indexlike(ctx, col_inds, index_bytes, n, 0, d_col, 4, s));
+        if (n) SPRS_CUDA(ctx, cudaMemcpyAsync(d_val, data, n * 8, cudaMemcpyHostToDevice, s));
+        SPRS_TRY(triplets_to_csr_launch(ctx, rows, cols, n, d_row, d_col, d_val, &t, s));
+    }
+    return finish_result(ctx, t, s, "from_triplets", true, out);
 }
 
 int sprs_b200_csmat_check_structure(sprs_b200_ctx* ctx, const sprs_b200_csmat* m,
@@ -575,19 +470,9 @@ int sprs_b200_csmat_to_other_storage(sprs_b200_ctx* ctx, const sprs_b200_csmat* 
     if (!ctx || !m || !out) return SPRS_B200_ERR_ARGUMENT;
     *out = nullptr;
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
-    auto* t = new sprs_b200_csmat();
-    int st = transpose_launch(ctx, m, t, ctx->stream);
-    if (st == SPRS_B200_OK) st = spmv_prepare(ctx, t, ctx->stream);
-    if (st == SPRS_B200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-        sprs_b200_set_error(ctx, "to_other_storage: kernel failed");
-        st = SPRS_B200_ERR_CUDA;
-    }
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(t);
-        return st;
-    }
-    *out = t;
-    return SPRS_B200_OK;
+    CsmatPtr t;
+    SPRS_TRY(transpose_launch(ctx, m, &t, ctx->stream));
+    return finish_result(ctx, t, ctx->stream, "to_other_storage", true, out);
 }
 
 // ---------------------------------------------------------------------------------
@@ -663,53 +548,37 @@ static int spmv_host(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, int want_st
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     const sprs_b200_csmat* csr = nullptr;
-    SPRS_TRY(csr_of(ctx, mat, &csr));
-    int st = SPRS_B200_OK;
-    do {
-        void *d_x = nullptr, *d_y = nullptr;
-        if ((st = ctx_scratch(ctx, 1, x_len * sizeof(double), &d_x)) != SPRS_B200_OK) break;
-        if ((st = ctx_scratch(ctx, 2, y_len * sizeof(double), &d_y)) != SPRS_B200_OK) break;
-        cudaError_t e = cudaSuccess;
-        if (x_len) e = cudaMemcpyAsync(d_x, x, x_len * sizeof(double), cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess && accumulate && y_len)
-            e = cudaMemcpyAsync(d_y, y, y_len * sizeof(double), cudaMemcpyHostToDevice, s);
-        if (e != cudaSuccess) {
-            sprs_b200_set_error(ctx, cudaGetErrorString(e));
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        // SPRS_B200_E2E_CHUNKS=n (n > 1): the tile stream runs in n chunks and each chunk's
-        // finished rows leave for the host behind its event while the next chunk computes
-        // (spmv_host_chunked); default: one launch, one D2H copy.
-        static const int chunks = [] {
-            const char* v = getenv("SPRS_B200_E2E_CHUNKS");
-            return v ? atoi(v) : SPRS_E2E_DEFAULT_CHUNKS;
-        }();
-        // (a chunk is worth its launch only with >= ~1000 tiles; SPRS_B200_E2E_MIN_TILES is a TEST
-        // hook that lets small matrices take the chunked path)
-        static const uint64_t min_tiles = [] {
-            const char* v = getenv("SPRS_B200_E2E_MIN_TILES");
-            return v ? (uint64_t)atoll(v) : (uint64_t)1024;
-        }();
-        if (chunks > 1 && y_len >= 4096 && csr->n_tiles >= (uint64_t)chunks * min_tiles) {
-            if ((st = spmv_host_chunked(ctx, csr, (const double*)d_x, (double*)d_y, y, accumulate,
-                                        chunks, s)) != SPRS_B200_OK)
-                break;
-            e = cudaStreamSynchronize(s);
-        } else {
-            if ((st = spmv_launch(ctx, csr, (const double*)d_x, (double*)d_y, accumulate, s)) !=
-                SPRS_B200_OK)
-                break;
-            if (y_len)
-                e = cudaMemcpyAsync(y, d_y, y_len * sizeof(double), cudaMemcpyDeviceToHost, s);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        }
-        if (e != cudaSuccess) {
-            sprs_b200_set_error(ctx, cudaGetErrorString(e));
-            st = SPRS_B200_ERR_CUDA;
-        }
-    } while (0);
-    return st;
+    SPRS_TRY(csmat_csr_view(ctx, mat, &csr));
+    void *d_x = nullptr, *d_y = nullptr;
+    SPRS_TRY(ctx_scratch(ctx, 1, x_len * sizeof(double), &d_x));
+    SPRS_TRY(ctx_scratch(ctx, 2, y_len * sizeof(double), &d_y));
+    if (x_len)
+        SPRS_CUDA(ctx, cudaMemcpyAsync(d_x, x, x_len * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (accumulate && y_len)
+        SPRS_CUDA(ctx, cudaMemcpyAsync(d_y, y, y_len * sizeof(double), cudaMemcpyHostToDevice, s));
+    // SPRS_B200_E2E_CHUNKS=n (n > 1): the tile stream runs in n chunks and each chunk's
+    // finished rows leave for the host behind its event while the next chunk computes
+    // (spmv_host_chunked); default: one launch, one D2H copy.
+    static const int chunks = [] {
+        const char* v = getenv("SPRS_B200_E2E_CHUNKS");
+        return v ? atoi(v) : SPRS_E2E_DEFAULT_CHUNKS;
+    }();
+    // (a chunk is worth its launch only with >= ~1000 tiles; SPRS_B200_E2E_MIN_TILES is a TEST
+    // hook that lets small matrices take the chunked path)
+    static const uint64_t min_tiles = [] {
+        const char* v = getenv("SPRS_B200_E2E_MIN_TILES");
+        return v ? (uint64_t)atoll(v) : (uint64_t)1024;
+    }();
+    if (chunks > 1 && y_len >= 4096 && csr->n_tiles >= (uint64_t)chunks * min_tiles) {
+        SPRS_TRY(spmv_host_chunked(ctx, csr, (const double*)d_x, (double*)d_y, y, accumulate,
+                                   chunks, s));
+    } else {
+        SPRS_TRY(spmv_launch(ctx, csr, (const double*)d_x, (double*)d_y, accumulate, s));
+        if (y_len)
+            SPRS_CUDA(ctx, cudaMemcpyAsync(y, d_y, y_len * sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+    SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+    return SPRS_B200_OK;
 }
 
 int sprs_b200_mul_acc_mat_vec_csr(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat,
@@ -746,68 +615,52 @@ static int dense_host(sprs_b200_ctx* ctx, const sprs_b200_csmat* lhs, int want_s
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     const sprs_b200_csmat* csr = nullptr;
-    SPRS_TRY(csr_of(ctx, lhs, &csr));
+    SPRS_TRY(csmat_csr_view(ctx, lhs, &csr));
     // Pack views on the host into the pinned staging buffer in the kernel's layout:
     // row-major (rowmaj) or column-major (colmaj).  O(size) copies, no arithmetic.
     const size_t nb = (size_t)rhs_rows * k, nc = (size_t)out_rows * k;
-    int st = SPRS_B200_OK;
-    do {
-        void* hs = nullptr;
-        if ((st = ctx_stage(ctx, (nb + nc) * sizeof(double), &hs)) != SPRS_B200_OK) break;
-        double* hb = (double*)hs;
-        double* hc = hb + nb;
-        if (rowmaj) {
+    void* hs = nullptr;
+    SPRS_TRY(ctx_stage(ctx, (nb + nc) * sizeof(double), &hs));
+    double* hb = (double*)hs;
+    double* hc = hb + nb;
+    if (rowmaj) {
+        for (uint64_t r = 0; r < rhs_rows; ++r)
+            for (uint64_t c = 0; c < k; ++c)
+                hb[r * k + c] = rhs[(int64_t)r * rhs_rs + (int64_t)c * rhs_cs];
+        for (uint64_t r = 0; r < out_rows; ++r)
+            for (uint64_t c = 0; c < k; ++c)
+                hc[r * k + c] = out[(int64_t)r * out_rs + (int64_t)c * out_cs];
+    } else {
+        for (uint64_t c = 0; c < k; ++c)
             for (uint64_t r = 0; r < rhs_rows; ++r)
-                for (uint64_t c = 0; c < k; ++c)
-                    hb[r * k + c] = rhs[(int64_t)r * rhs_rs + (int64_t)c * rhs_cs];
+                hb[c * rhs_rows + r] = rhs[(int64_t)r * rhs_rs + (int64_t)c * rhs_cs];
+        for (uint64_t c = 0; c < k; ++c)
             for (uint64_t r = 0; r < out_rows; ++r)
-                for (uint64_t c = 0; c < k; ++c)
-                    hc[r * k + c] = out[(int64_t)r * out_rs + (int64_t)c * out_cs];
-        } else {
+                hc[c * out_rows + r] = out[(int64_t)r * out_rs + (int64_t)c * out_cs];
+    }
+    void *d_b = nullptr, *d_c = nullptr;
+    SPRS_TRY(ctx_scratch(ctx, 1, nb * sizeof(double), &d_b));
+    SPRS_TRY(ctx_scratch(ctx, 2, nc * sizeof(double), &d_c));
+    SPRS_CUDA(ctx, cudaMemcpyAsync(d_b, hb, nb * sizeof(double), cudaMemcpyHostToDevice, s));
+    SPRS_CUDA(ctx, cudaMemcpyAsync(d_c, hc, nc * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (rowmaj)
+        SPRS_TRY(spmm_rowmaj_launch(ctx, csr, (const double*)d_b, k, k, (double*)d_c, k, 1, s));
+    else
+        for (uint64_t c = 0; c < k; ++c)
+            SPRS_TRY(spmv_launch(ctx, csr, (const double*)d_b + c * rhs_rows,
+                                 (double*)d_c + c * out_rows, 1, s));
+    SPRS_CUDA(ctx, cudaMemcpyAsync(hc, d_c, nc * sizeof(double), cudaMemcpyDeviceToHost, s));
+    SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+    if (rowmaj) {
+        for (uint64_t r = 0; r < out_rows; ++r)
             for (uint64_t c = 0; c < k; ++c)
-                for (uint64_t r = 0; r < rhs_rows; ++r)
-                    hb[c * rhs_rows + r] = rhs[(int64_t)r * rhs_rs + (int64_t)c * rhs_cs];
-            for (uint64_t c = 0; c < k; ++c)
-                for (uint64_t r = 0; r < out_rows; ++r)
-                    hc[c * out_rows + r] = out[(int64_t)r * out_rs + (int64_t)c * out_cs];
-        }
-        void *d_b = nullptr, *d_c = nullptr;
-        if ((st = ctx_scratch(ctx, 1, nb * sizeof(double), &d_b)) != SPRS_B200_OK) break;
-        if ((st = ctx_scratch(ctx, 2, nc * sizeof(double), &d_c)) != SPRS_B200_OK) break;
-        cudaError_t e = cudaMemcpyAsync(d_b, hb, nb * sizeof(double), cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess)
-            e = cudaMemcpyAsync(d_c, hc, nc * sizeof(double), cudaMemcpyHostToDevice, s);
-        if (e != cudaSuccess) {
-            sprs_b200_set_error(ctx, cudaGetErrorString(e));
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        if (rowmaj) {
-            st = spmm_rowmaj_launch(ctx, csr, (const double*)d_b, k, k, (double*)d_c, k, 1, s);
-        } else {
-            for (uint64_t c = 0; c < k && st == SPRS_B200_OK; ++c)
-                st = spmv_launch(ctx, csr, (const double*)d_b + c * rhs_rows,
-                                 (double*)d_c + c * out_rows, 1, s);
-        }
-        if (st != SPRS_B200_OK) break;
-        e = cudaMemcpyAsync(hc, d_c, nc * sizeof(double), cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) {
-            sprs_b200_set_error(ctx, cudaGetErrorString(e));
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        if (rowmaj) {
+                out[(int64_t)r * out_rs + (int64_t)c * out_cs] = hc[r * k + c];
+    } else {
+        for (uint64_t c = 0; c < k; ++c)
             for (uint64_t r = 0; r < out_rows; ++r)
-                for (uint64_t c = 0; c < k; ++c)
-                    out[(int64_t)r * out_rs + (int64_t)c * out_cs] = hc[r * k + c];
-        } else {
-            for (uint64_t c = 0; c < k; ++c)
-                for (uint64_t r = 0; r < out_rows; ++r)
-                    out[(int64_t)r * out_rs + (int64_t)c * out_cs] = hc[c * out_rows + r];
-        }
-    } while (0);
-    return st;
+                out[(int64_t)r * out_rs + (int64_t)c * out_cs] = hc[c * out_rows + r];
+    }
+    return SPRS_B200_OK;
 }
 
 int sprs_b200_csr_mulacc_dense_rowmaj(sprs_b200_ctx* ctx, const sprs_b200_csmat* lhs,
@@ -845,55 +698,89 @@ int sprs_b200_csc_mulacc_dense_colmaj(sprs_b200_ctx* ctx, const sprs_b200_csmat*
 
 }  // extern "C"
 
-// ---- device-built results (declared in common.cuh): the binops, scale, construct.cu and
-// the dense boundary in transpose.cu build their result mirrors with these
-bool force_indptr64() {
-    // the SPRS_B200_FORCE_INDPTR64 test hook of csmat_upload, applied to the results too
+// ---- scoped ownership and mirrors built on the device (declared in common.cuh)
+int mem_alloc(sprs_b200_ctx* ctx, MemKind kind, size_t bytes, cudaStream_t s, const char* what,
+              void** p) {
+    const cudaError_t e = kind == MemKind::device   ? cudaMalloc(p, bytes)
+                          : kind == MemKind::stream ? cudaMallocAsync(p, bytes, s)
+                                                    : cudaMallocHost(p, bytes);
+    if (e == cudaSuccess) return SPRS_B200_OK;
+    cudaGetLastError();  // (the failed allocation leaves its error behind: reported here)
+    *p = nullptr;
+    static const char* const calls[] = {"cudaMalloc", "cudaMallocAsync", "cudaMallocHost"};
+    SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "%s: %s of %zu bytes failed: %s", what, calls[(int)kind],
+              bytes, cudaGetErrorString(e));
+}
+
+void mem_free(MemKind kind, void* p, cudaStream_t s) {
+    if (kind == MemKind::device)
+        cudaFree(p);
+    else if (kind == MemKind::stream)
+        cudaFreeAsync(p, s);
+    else
+        cudaFreeHost(p);
+}
+
+int indptr_bytes_for(uint64_t nnz) {
     static const bool force64 = [] {
         const char* v = getenv("SPRS_B200_FORCE_INDPTR64");
         return v && atoi(v) != 0;
     }();
-    return force64;
+    return (nnz >= 0xffffffffull || force64) ? 8 : 4;
 }
 
-sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
-                            uint64_t nnz, int indptr_bytes) {
-    auto* m = new sprs_b200_csmat();
-    m->ctx = ctx;
-    m->storage = storage;
-    m->rows = rows;
-    m->cols = cols;
-    m->outer = storage == SPRS_B200_CSR ? rows : cols;
-    m->inner = storage == SPRS_B200_CSR ? cols : rows;
-    m->nnz = nnz;
-    m->indptr_bytes = indptr_bytes;
-    m->pooled = true;
+sprs_b200_csmat csmat_init(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
+                           uint64_t nnz, int indptr_bytes, Arrays arrays) {
+    sprs_b200_csmat m;
+    m.ctx = ctx;
+    m.storage = storage;
+    m.rows = rows;
+    m.cols = cols;
+    m.outer = storage == SPRS_B200_CSR ? rows : cols;
+    m.inner = storage == SPRS_B200_CSR ? cols : rows;
+    m.nnz = nnz;
+    m.indptr_bytes = indptr_bytes;
+    m.owns = arrays != Arrays::borrowed;
+    m.pooled = arrays == Arrays::pooled;
     return m;
 }
 
-sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, const sprs_b200_csmat* like, uint64_t nnz,
-                            int indptr_bytes) {
-    return new_result(ctx, like->storage, like->rows, like->cols, nnz, indptr_bytes);
+CsmatPtr new_result(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols, uint64_t nnz,
+                    int indptr_bytes, Arrays arrays) {
+    return CsmatPtr(new sprs_b200_csmat(
+        csmat_init(ctx, storage, rows, cols, nnz, indptr_bytes, arrays)));
 }
 
-int alloc_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s) {
-    if (cudaMallocAsync(&m->d_indptr, (m->outer + 1) * (size_t)m->indptr_bytes + 16, s) != cudaSuccess ||
-        cudaMallocAsync((void**)&m->d_indices, m->nnz * 4 + 16, s) != cudaSuccess ||
-        cudaMallocAsync((void**)&m->d_data, m->nnz * 8 + 16, s) != cudaSuccess) {
-        cudaGetLastError();
-        SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "binop: cudaMallocAsync of the result failed");
-    }
+int alloc_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, const char* what) {
+    const MemKind kind = m->pooled ? MemKind::stream : MemKind::device;
+    SPRS_TRY(mem_alloc(ctx, kind, (m->outer + 1) * (size_t)m->indptr_bytes + 16, s, what,
+                       &m->d_indptr));
+    SPRS_TRY(mem_alloc(ctx, kind, m->nnz * 4 + 16, s, what, (void**)&m->d_indices));
+    SPRS_TRY(mem_alloc(ctx, kind, m->nnz * 8 + 16, s, what, (void**)&m->d_data));
     return SPRS_B200_OK;
 }
 
-// The result's SpMV partition (no hot set: its build would run inside every call), then wait.
-int finish_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, const char* what) {
-    SPRS_TRY(spmv_prepare(ctx, m, s, false));
+// CSR view of a mirror for the product kernels: the mirror itself, or (CSC) its cached
+// device conversion -- same sums in the same order (ascending column per output element).
+int csmat_csr_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const sprs_b200_csmat** out) {
+    if (m->storage == SPRS_B200_CSR) {
+        *out = m;
+        return SPRS_B200_OK;
+    }
+    if (!m->csr_cache) {
+        sprs_b200_csmat* t = nullptr;
+        SPRS_TRY(sprs_b200_csmat_to_other_storage(ctx, m, &t));
+        m->csr_cache = t;
+    }
+    *out = m->csr_cache;
+    return SPRS_B200_OK;
+}
+
+int finish_result(sprs_b200_ctx* ctx, CsmatPtr& m, cudaStream_t s, const char* what, bool hot_set,
+                  sprs_b200_csmat** out) {
+    SPRS_TRY(spmv_prepare(ctx, m.get(), s, hot_set));
     if (cudaStreamSynchronize(s) != cudaSuccess || cudaGetLastError() != cudaSuccess)
         SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "%s: kernel failed", what);
+    *out = m.release();
     return SPRS_B200_OK;
-}
-
-int csmat_csr_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const sprs_b200_csmat** out) {
-    return csr_of(ctx, m, out);
 }

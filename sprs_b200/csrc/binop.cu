@@ -245,70 +245,40 @@ int run_binop(sprs_b200_ctx* ctx, const sprs_b200_csmat* a, const sprs_b200_csma
     const uint64_t total = a->nnz + b->nnz + BINOP_ROW_COST * a->outer;
     const uint64_t n_tiles = (total + BINOP_TILE - 1) / BINOP_TILE;
     const uint64_t n_lanes = n_tiles * 32;
-    uint32_t *cut_r = nullptr, *lane_cnt = nullptr;
-    uint64_t *cut_a = nullptr, *cut_b = nullptr, *lane_off = nullptr;
-    sprs_b200_csmat* c = nullptr;
-    int st = SPRS_B200_OK;
-    do {
-        uint64_t nnz_c = 0;
-        if (n_tiles) {
-            if (cudaMallocAsync((void**)&cut_r, (n_tiles + 1) * 4, s) != cudaSuccess ||
-                cudaMallocAsync((void**)&cut_a, (n_tiles + 1) * 8, s) != cudaSuccess ||
-                cudaMallocAsync((void**)&cut_b, (n_tiles + 1) * 8, s) != cudaSuccess ||
-                cudaMallocAsync((void**)&lane_cnt, n_lanes * 4, s) != cudaSuccess ||
-                cudaMallocAsync((void**)&lane_off, (n_lanes + 1) * 8, s) != cudaSuccess) {
-                cudaGetLastError();
-                sprs_b200_set_error(ctx, "binop: cudaMallocAsync of the partition failed");
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-            binop_cut_kernel<PA, PB><<<(unsigned)((n_tiles + 1 + 255) / 256), 256, 0, s>>>(
-                o, total, n_tiles, cut_r, cut_a, cut_b);
-            binop_count_kernel<PA, PB><<<(unsigned)((n_tiles + 7) / 8), 256, 0, s>>>(
-                o, op, total, n_tiles, cut_r, cut_a, cut_b, lane_cnt);
-            ctx->launches += 2;
-            if ((st = device_exclusive_scan<uint32_t, uint64_t>(ctx, lane_cnt, n_lanes, lane_off,
-                                                                s)) != SPRS_B200_OK)
-                break;
-            if (cudaMemcpyAsync(&nnz_c, lane_off + n_lanes, 8, cudaMemcpyDeviceToHost, s) !=
-                    cudaSuccess ||
-                cudaStreamSynchronize(s) != cudaSuccess) {
-                sprs_b200_set_error(ctx, "binop: count pass failed");
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-        }
-        c = new_result(ctx, a, nnz_c, (nnz_c >= 0xffffffffull || force_indptr64()) ? 8 : 4);
-        if ((st = alloc_result(ctx, c, s)) != SPRS_B200_OK) break;
-        if (n_tiles == 0) {  // no outer dimension: indptr = [0]
-            if (cudaMemsetAsync(c->d_indptr, 0, c->indptr_bytes, s) != cudaSuccess) {
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-        } else if (c->indptr_bytes == 4) {
-            launch_fill<PA, PB, uint32_t>(o, op, total, n_tiles, cut_r, cut_a, cut_b, lane_off, c, s);
-        } else {
-            launch_fill<PA, PB, uint64_t>(o, op, total, n_tiles, cut_r, cut_a, cut_b, lane_off, c, s);
-        }
-        ctx->launches += n_tiles ? 1 : 0;
-        if (cudaGetLastError() != cudaSuccess) {
-            sprs_b200_set_error(ctx, "binop: launch failed");
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        st = finish_result(ctx, c, s, "binop");
-    } while (0);
-    if (cut_r) cudaFreeAsync(cut_r, s);
-    if (cut_a) cudaFreeAsync(cut_a, s);
-    if (cut_b) cudaFreeAsync(cut_b, s);
-    if (lane_cnt) cudaFreeAsync(lane_cnt, s);
-    if (lane_off) cudaFreeAsync(lane_off, s);
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(c);
-        return st;
+    uint64_t nnz_c = 0;
+    Owned<uint32_t> cut_r, lane_cnt;
+    Owned<uint64_t> cut_a, cut_b, lane_off;
+    if (n_tiles) {
+        SPRS_TRY(cut_r.alloc_async(ctx, (n_tiles + 1) * 4, s, "binop"));
+        SPRS_TRY(cut_a.alloc_async(ctx, (n_tiles + 1) * 8, s, "binop"));
+        SPRS_TRY(cut_b.alloc_async(ctx, (n_tiles + 1) * 8, s, "binop"));
+        SPRS_TRY(lane_cnt.alloc_async(ctx, n_lanes * 4, s, "binop"));
+        SPRS_TRY(lane_off.alloc_async(ctx, (n_lanes + 1) * 8, s, "binop"));
+        binop_cut_kernel<PA, PB><<<(unsigned)((n_tiles + 1 + 255) / 256), 256, 0, s>>>(
+            o, total, n_tiles, cut_r, cut_a, cut_b);
+        binop_count_kernel<PA, PB><<<(unsigned)((n_tiles + 7) / 8), 256, 0, s>>>(
+            o, op, total, n_tiles, cut_r, cut_a, cut_b, lane_cnt);
+        ctx->launches += 2;
+        SPRS_TRY((device_exclusive_scan<uint32_t, uint64_t>(ctx, lane_cnt, n_lanes, lane_off, s)));
+        if (cudaMemcpyAsync(&nnz_c, lane_off + n_lanes, 8, cudaMemcpyDeviceToHost, s) !=
+                cudaSuccess ||
+            cudaStreamSynchronize(s) != cudaSuccess)
+            SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "binop: count pass failed");
     }
-    *out = c;
-    return SPRS_B200_OK;
+    CsmatPtr c = new_result(ctx, a->storage, a->rows, a->cols, nnz_c, indptr_bytes_for(nnz_c),
+                            Arrays::pooled);
+    SPRS_TRY(alloc_result(ctx, c.get(), s, "binop"));
+    if (n_tiles == 0) {  // no outer dimension: indptr = [0]
+        if (cudaMemsetAsync(c->d_indptr, 0, c->indptr_bytes, s) != cudaSuccess)
+            SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "binop: memset failed");
+    } else if (c->indptr_bytes == 4) {
+        launch_fill<PA, PB, uint32_t>(o, op, total, n_tiles, cut_r, cut_a, cut_b, lane_off, c.get(), s);
+    } else {
+        launch_fill<PA, PB, uint64_t>(o, op, total, n_tiles, cut_r, cut_a, cut_b, lane_off, c.get(), s);
+    }
+    ctx->launches += n_tiles ? 1 : 0;
+    if (cudaGetLastError() != cudaSuccess) SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "binop: launch failed");
+    return finish_result(ctx, c, s, "binop", false, out);
 }
 
 }  // namespace
@@ -340,29 +310,22 @@ int sprs_b200_csmat_scale(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, double s
     *out = nullptr;
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
-    sprs_b200_csmat* c = new_result(ctx, m, m->nnz, m->indptr_bytes);
-    int st = alloc_result(ctx, c, s);
-    if (st == SPRS_B200_OK) {
-        const uint64_t n = m->nnz > m->outer + 1 ? m->nnz : m->outer + 1;
-        const unsigned grid = (unsigned)std::min<uint64_t>((n + 255) / 256,
-                                                           (uint64_t)ctx->sm_count * 16);
-        if (m->indptr_bytes == 4)
-            scale_kernel<uint32_t><<<grid, 256, 0, s>>>(
-                (const uint32_t*)m->d_indptr, m->d_indices, m->d_data, m->outer, m->nnz, s_val,
-                ctx->pol_evict_first, (uint32_t*)c->d_indptr, c->d_indices, c->d_data);
-        else
-            scale_kernel<uint64_t><<<grid, 256, 0, s>>>(
-                (const uint64_t*)m->d_indptr, m->d_indices, m->d_data, m->outer, m->nnz, s_val,
-                ctx->pol_evict_first, (uint64_t*)c->d_indptr, c->d_indices, c->d_data);
-        ctx->launches += 1;
-        st = finish_result(ctx, c, s, "scale");
-    }
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(c);
-        return st;
-    }
-    *out = c;
-    return SPRS_B200_OK;
+    CsmatPtr c = new_result(ctx, m->storage, m->rows, m->cols, m->nnz, m->indptr_bytes,
+                            Arrays::pooled);
+    SPRS_TRY(alloc_result(ctx, c.get(), s, "scale"));
+    const uint64_t n = m->nnz > m->outer + 1 ? m->nnz : m->outer + 1;
+    const unsigned grid = (unsigned)std::min<uint64_t>((n + 255) / 256,
+                                                       (uint64_t)ctx->sm_count * 16);
+    if (m->indptr_bytes == 4)
+        scale_kernel<uint32_t><<<grid, 256, 0, s>>>(
+            (const uint32_t*)m->d_indptr, m->d_indices, m->d_data, m->outer, m->nnz, s_val,
+            ctx->pol_evict_first, (uint32_t*)c->d_indptr, c->d_indices, c->d_data);
+    else
+        scale_kernel<uint64_t><<<grid, 256, 0, s>>>(
+            (const uint64_t*)m->d_indptr, m->d_indices, m->d_data, m->outer, m->nnz, s_val,
+            ctx->pol_evict_first, (uint64_t*)c->d_indptr, c->d_indices, c->d_data);
+    ctx->launches += 1;
+    return finish_result(ctx, c, s, "scale", false, out);
 }
 
 }  // extern "C"

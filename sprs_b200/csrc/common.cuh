@@ -5,6 +5,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -108,6 +109,70 @@ static inline cudaStream_t pick_stream(sprs_b200_ctx*, void* stream) {
 int ctx_scratch(sprs_b200_ctx* ctx, int i, size_t bytes, void** out);
 int ctx_stage(sprs_b200_ctx* ctx, size_t bytes, void** out);
 
+// ---- scoped ownership (host code) -----------------------------------------------
+// Where an owned allocation comes from: cudaMalloc, cudaMallocAsync (freed on the stream it was
+// allocated on) or cudaMallocHost.
+enum class MemKind { device, stream, pinned };
+// `bytes` of `kind` into *p.  On failure: clears the runtime's error, sets the ctx's last error
+// to "<what>: ..." and returns ERR_CUDA (api.cu).
+int mem_alloc(sprs_b200_ctx* ctx, MemKind kind, size_t bytes, cudaStream_t s, const char* what,
+              void** p);
+void mem_free(MemKind kind, void* p, cudaStream_t s);
+
+// One allocation, released when its owner goes out of scope (or on reset / the next alloc).
+template <typename T>
+class Owned {
+  public:
+    Owned() = default;
+    Owned(const Owned&) = delete;
+    Owned& operator=(const Owned&) = delete;
+    Owned(Owned&& o) noexcept : p_(o.release()), kind_(o.kind_), s_(o.s_) {}
+    ~Owned() { reset(); }
+
+    int alloc(sprs_b200_ctx* ctx, size_t bytes, const char* what) {
+        return take(ctx, MemKind::device, bytes, nullptr, what);
+    }
+    int alloc_async(sprs_b200_ctx* ctx, size_t bytes, cudaStream_t s, const char* what) {
+        return take(ctx, MemKind::stream, bytes, s, what);
+    }
+    int alloc_pinned(sprs_b200_ctx* ctx, size_t bytes, const char* what) {
+        return take(ctx, MemKind::pinned, bytes, nullptr, what);
+    }
+    void reset() {
+        if (p_) mem_free(kind_, p_, s_);
+        p_ = nullptr;
+    }
+    T* release() {
+        T* p = p_;
+        p_ = nullptr;
+        return p;
+    }
+    operator T*() const { return p_; }
+
+  private:
+    int take(sprs_b200_ctx* ctx, MemKind kind, size_t bytes, cudaStream_t s, const char* what) {
+        reset();
+        void* p = nullptr;
+        SPRS_TRY(mem_alloc(ctx, kind, bytes, s, what, &p));
+        p_ = (T*)p;
+        kind_ = kind;
+        s_ = s;
+        return SPRS_B200_OK;
+    }
+    T* p_ = nullptr;
+    MemKind kind_ = MemKind::device;
+    cudaStream_t s_ = nullptr;
+};
+
+// unique_ptr deleter that calls one of the library's free functions
+template <auto Free>
+struct FreeWith {
+    template <typename T>
+    void operator()(T* p) const { Free(p); }
+};
+// A mirror being built: freed by sprs_b200_csmat_free unless release()d into *out.
+using CsmatPtr = std::unique_ptr<sprs_b200_csmat, FreeWith<sprs_b200_csmat_free>>;
+
 // y targets of one SpMV: [0] = local y (already offset to this rank's first row), [1..n) =
 // the same position inside the peer GPUs' y buffers (CUDA IPC mappings).
 constexpr int SPMV_MAX_TARGETS = 8;
@@ -144,26 +209,31 @@ int spmm_rowmaj_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const doubl
                        cudaStream_t s);
 int triplets_to_csr_launch(sprs_b200_ctx* ctx, uint64_t rows, uint64_t cols, uint64_t n,
                            const uint32_t* d_row, const uint32_t* d_col, const double* d_val,
-                           sprs_b200_csmat* out, cudaStream_t s);
-int transpose_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, sprs_b200_csmat* out,
-                     cudaStream_t s);
+                           CsmatPtr* out, cudaStream_t s);
+int transpose_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, CsmatPtr* out, cudaStream_t s);
 // CSR form of a mirror for the product kernels: the mirror itself or (CSC) its cached
 // device conversion, owned by the mirror (api.cu)
 int csmat_csr_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, const sprs_b200_csmat** out);
 
-// ---- device-built results (api.cu; the binops, scale, construct.cu and the dense boundary in transpose.cu use them)
-// the SPRS_B200_FORCE_INDPTR64 test hook of csmat_upload, applied to the results too
-bool force_indptr64();
-// a pooled result mirror with like's storage and shape (no arrays yet)
-sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, const sprs_b200_csmat* like, uint64_t nnz,
-                            int indptr_bytes);
-// the same with the storage and shape given
-sprs_b200_csmat* new_result(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
-                            uint64_t nnz, int indptr_bytes);
-// its indptr / indices / data, stream-ordered on s
-int alloc_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s);
-// its SpMV partition (no hot set), then wait for s
-int finish_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, const char* what);
+// ---- mirrors built on the device (api.cu) -----------------------------------------
+// Who holds a mirror's arrays: cudaMalloc (owned), cudaMallocAsync on the ctx stream (pooled)
+// or the caller (borrowed).
+enum class Arrays { owned, pooled, borrowed };
+// The initialiser of every mirror: storage, shape, nnz, indptr width, who holds the arrays
+sprs_b200_csmat csmat_init(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
+                           uint64_t nnz, int indptr_bytes, Arrays arrays);
+// the same on the heap (no arrays yet)
+CsmatPtr new_result(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols, uint64_t nnz,
+                    int indptr_bytes, Arrays arrays);
+// 4, or 8 where nnz needs it.  SPRS_B200_FORCE_INDPTR64=1 is a TEST hook: 8 always, so that
+// the uint64 instantiations of the kernels run at sizes a test can afford.
+int indptr_bytes_for(uint64_t nnz);
+// a new mirror's indptr / indices / data, stream-ordered on s where it is pooled
+int alloc_result(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, const char* what);
+// The finishing step of a new mirror: its SpMV partition (hot_set: and the hot set where it
+// pays), then wait for s; on success m is handed out through *out.
+int finish_result(sprs_b200_ctx* ctx, CsmatPtr& m, cudaStream_t s, const char* what, bool hot_set,
+                  sprs_b200_csmat** out);
 
 // ---- small device helpers -----------------------------------------------------
 #ifdef __CUDACC__

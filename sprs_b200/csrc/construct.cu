@@ -29,7 +29,7 @@
 //               rows at once (one lane reads each row's indptr entries, so the reads overlap)
 //               and each output entry finds its row by a 5-step shuffle search over the lanes'
 //               row starts.  Index ja*inner(b) + jb in 64 bits, value __dmul_rn(va, vb).
-//   * Results come from new_result / alloc_result / finish_result (binop.cu): stream-ordered
+//   * Results come from new_result / alloc_result / finish_result (api.cu): stream-ordered
 //     pool arrays, 64-bit indptr exactly when nnz >= 2^32 - 1 (or SPRS_B200_FORCE_INDPTR64),
 //     the SpMV partition built.  No atomics, no waits between CTAs: deterministic.
 //   * Every contract check runs on the host before any device work.
@@ -274,18 +274,6 @@ unsigned grid_for(const sprs_b200_ctx* ctx, uint64_t n) {
         1, std::min<uint64_t>((n + 255) / 256, (uint64_t)ctx->sm_count * 16));
 }
 
-// a pooled result mirror of the given storage and shape
-sprs_b200_csmat* construct_result(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols,
-                                  uint64_t nnz) {
-    sprs_b200_csmat like;
-    like.storage = storage;
-    like.rows = rows;
-    like.cols = cols;
-    like.outer = storage == SPRS_B200_CSR ? rows : cols;
-    like.inner = storage == SPRS_B200_CSR ? cols : rows;
-    return new_result(ctx, &like, nnz, (nnz >= 0xffffffffull || force_indptr64()) ? 8 : 4);
-}
-
 bool mul_overflows(uint64_t a, uint64_t b, uint64_t* out) {
     return __builtin_mul_overflow(a, b, out);
 }
@@ -368,61 +356,45 @@ int sprs_b200_csmat_bmat(sprs_b200_ctx* ctx, uint64_t n_block_rows, uint64_t n_b
     }
     first[nbr] = blk.size();
 
-    sprs_b200_csmat* c = construct_result(ctx, SPRS_B200_CSR, rows, width0, nnz);
-    void* d_table = nullptr;
-    int st = SPRS_B200_OK;
-    do {
-        if ((st = alloc_result(ctx, c, s)) != SPRS_B200_OK) break;
-        const size_t blk_bytes = blk.size() * sizeof(Block), tab_bytes = (nbr + 1) * 8;
-        std::vector<unsigned char> host(blk_bytes + 3 * tab_bytes);
-        memcpy(host.data(), blk.data(), blk_bytes);
-        memcpy(host.data() + blk_bytes, row0.data(), tab_bytes);
-        memcpy(host.data() + blk_bytes + tab_bytes, base.data(), tab_bytes);
-        memcpy(host.data() + blk_bytes + 2 * tab_bytes, first.data(), tab_bytes);
-        if (cudaMallocAsync(&d_table, host.size(), s) != cudaSuccess ||
-            cudaMemcpyAsync(d_table, host.data(), host.size(), cudaMemcpyHostToDevice, s) !=
-                cudaSuccess) {
-            cudaGetLastError();
-            sprs_b200_set_error(ctx, "bmat: upload of the block table failed");
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        const unsigned char* d = (const unsigned char*)d_table;
-        const Table t{(const Block*)d, (const uint64_t*)(d + blk_bytes),
-                      (const uint64_t*)(d + blk_bytes + tab_bytes),
-                      (const uint64_t*)(d + blk_bytes + 2 * tab_bytes), nbr};
-        const uint64_t n_tiles = (nnz + CONSTRUCT_TILE - 1) / CONSTRUCT_TILE;
-        const unsigned fill_grid = (unsigned)((n_tiles + 7) / 8);
-        if (c->indptr_bytes == 4) {
-            bmat_indptr_kernel<uint32_t><<<grid_for(ctx, rows + 1), 256, 0, s>>>(
-                t, rows, (uint32_t*)c->d_indptr);
-            if (n_tiles)
-                bmat_fill_kernel<uint32_t><<<fill_grid, 256, 0, s>>>(
-                    t, rows, nnz, n_tiles, (const uint32_t*)c->d_indptr, c->d_indices,
-                    (unsigned long long*)c->d_data);
-        } else {
-            bmat_indptr_kernel<uint64_t><<<grid_for(ctx, rows + 1), 256, 0, s>>>(
-                t, rows, (uint64_t*)c->d_indptr);
-            if (n_tiles)
-                bmat_fill_kernel<uint64_t><<<fill_grid, 256, 0, s>>>(
-                    t, rows, nnz, n_tiles, (const uint64_t*)c->d_indptr, c->d_indices,
-                    (unsigned long long*)c->d_data);
-        }
-        ctx->launches += n_tiles ? 2 : 1;
-        if (cudaGetLastError() != cudaSuccess) {
-            sprs_b200_set_error(ctx, "bmat: launch failed");
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        st = finish_result(ctx, c, s, "bmat");
-    } while (0);
-    if (d_table) cudaFreeAsync(d_table, s);
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(c);
-        return st;
+    CsmatPtr c = new_result(ctx, SPRS_B200_CSR, rows, width0, nnz, indptr_bytes_for(nnz),
+                            Arrays::pooled);
+    SPRS_TRY(alloc_result(ctx, c.get(), s, "bmat"));
+    const size_t blk_bytes = blk.size() * sizeof(Block), tab_bytes = (nbr + 1) * 8;
+    std::vector<unsigned char> host(blk_bytes + 3 * tab_bytes);
+    memcpy(host.data(), blk.data(), blk_bytes);
+    memcpy(host.data() + blk_bytes, row0.data(), tab_bytes);
+    memcpy(host.data() + blk_bytes + tab_bytes, base.data(), tab_bytes);
+    memcpy(host.data() + blk_bytes + 2 * tab_bytes, first.data(), tab_bytes);
+    Owned<unsigned char> d_table;
+    SPRS_TRY(d_table.alloc_async(ctx, host.size(), s, "bmat"));
+    if (cudaMemcpyAsync(d_table, host.data(), host.size(), cudaMemcpyHostToDevice, s) != cudaSuccess) {
+        cudaGetLastError();
+        SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "bmat: upload of the block table failed");
     }
-    *out = c;
-    return SPRS_B200_OK;
+    const unsigned char* d = d_table;
+    const Table t{(const Block*)d, (const uint64_t*)(d + blk_bytes),
+                  (const uint64_t*)(d + blk_bytes + tab_bytes),
+                  (const uint64_t*)(d + blk_bytes + 2 * tab_bytes), nbr};
+    const uint64_t n_tiles = (nnz + CONSTRUCT_TILE - 1) / CONSTRUCT_TILE;
+    const unsigned fill_grid = (unsigned)((n_tiles + 7) / 8);
+    if (c->indptr_bytes == 4) {
+        bmat_indptr_kernel<uint32_t><<<grid_for(ctx, rows + 1), 256, 0, s>>>(
+            t, rows, (uint32_t*)c->d_indptr);
+        if (n_tiles)
+            bmat_fill_kernel<uint32_t><<<fill_grid, 256, 0, s>>>(
+                t, rows, nnz, n_tiles, (const uint32_t*)c->d_indptr, c->d_indices,
+                (unsigned long long*)c->d_data);
+    } else {
+        bmat_indptr_kernel<uint64_t><<<grid_for(ctx, rows + 1), 256, 0, s>>>(
+            t, rows, (uint64_t*)c->d_indptr);
+        if (n_tiles)
+            bmat_fill_kernel<uint64_t><<<fill_grid, 256, 0, s>>>(
+                t, rows, nnz, n_tiles, (const uint64_t*)c->d_indptr, c->d_indices,
+                (unsigned long long*)c->d_data);
+    }
+    ctx->launches += n_tiles ? 2 : 1;
+    if (cudaGetLastError() != cudaSuccess) SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "bmat: launch failed");
+    return finish_result(ctx, c, s, "bmat", false, out);
 }
 
 int sprs_b200_csmat_kron(sprs_b200_ctx* ctx, const sprs_b200_csmat* a, const sprs_b200_csmat* b,
@@ -441,54 +413,40 @@ int sprs_b200_csmat_kron(sprs_b200_ctx* ctx, const sprs_b200_csmat* a, const spr
     cudaStream_t s = ctx->stream;
     // kronecker.rs: b in a's storage (to_other_storage); a CSR mirror's CSC b uses its cache
     const sprs_b200_csmat* bb = b;
-    sprs_b200_csmat* owned = nullptr;
+    sprs_b200_csmat* converted = nullptr;
     if (b->storage != a->storage) {
         if (a->storage == SPRS_B200_CSR) {
             SPRS_TRY(csmat_csr_view(ctx, b, &bb));
         } else {
-            SPRS_TRY(sprs_b200_csmat_to_other_storage(ctx, b, &owned));
-            bb = owned;
+            SPRS_TRY(sprs_b200_csmat_to_other_storage(ctx, b, &converted));
+            bb = converted;
         }
     }
+    const CsmatPtr owned(converted);
     const uint64_t outer_c = a->outer * bb->outer;
-    sprs_b200_csmat* c = construct_result(ctx, a->storage, rows, cols, nnz);
+    CsmatPtr c = new_result(ctx, a->storage, rows, cols, nnz, indptr_bytes_for(nnz), Arrays::pooled);
     const KronOperands o{a->d_indptr, a->d_indices, a->d_data, bb->d_indptr, bb->d_indices,
                          bb->d_data, bb->outer, bb->inner, bb->nnz,
                          a->indptr_bytes == 8 ? 1u : 0u, bb->indptr_bytes == 8 ? 1u : 0u};
-    int st = alloc_result(ctx, c, s);
-    if (st == SPRS_B200_OK) {
-        const uint64_t n_tiles = (nnz + CONSTRUCT_TILE - 1) / CONSTRUCT_TILE;
-        const unsigned fill_grid = (unsigned)((n_tiles + 7) / 8);
-        if (c->indptr_bytes == 4) {
-            kron_indptr_kernel<uint32_t><<<grid_for(ctx, outer_c + 1), 256, 0, s>>>(
-                o, outer_c, nnz, (uint32_t*)c->d_indptr);
-            if (n_tiles)
-                kron_fill_kernel<uint32_t><<<fill_grid, 256, 0, s>>>(
-                    o, outer_c, nnz, n_tiles, (const uint32_t*)c->d_indptr, c->d_indices,
-                    c->d_data);
-        } else {
-            kron_indptr_kernel<uint64_t><<<grid_for(ctx, outer_c + 1), 256, 0, s>>>(
-                o, outer_c, nnz, (uint64_t*)c->d_indptr);
-            if (n_tiles)
-                kron_fill_kernel<uint64_t><<<fill_grid, 256, 0, s>>>(
-                    o, outer_c, nnz, n_tiles, (const uint64_t*)c->d_indptr, c->d_indices,
-                    c->d_data);
-        }
-        ctx->launches += n_tiles ? 2 : 1;
-        if (cudaGetLastError() != cudaSuccess) {
-            sprs_b200_set_error(ctx, "kron: launch failed");
-            st = SPRS_B200_ERR_CUDA;
-        } else {
-            st = finish_result(ctx, c, s, "kron");
-        }
+    SPRS_TRY(alloc_result(ctx, c.get(), s, "kron"));
+    const uint64_t n_tiles = (nnz + CONSTRUCT_TILE - 1) / CONSTRUCT_TILE;
+    const unsigned fill_grid = (unsigned)((n_tiles + 7) / 8);
+    if (c->indptr_bytes == 4) {
+        kron_indptr_kernel<uint32_t><<<grid_for(ctx, outer_c + 1), 256, 0, s>>>(
+            o, outer_c, nnz, (uint32_t*)c->d_indptr);
+        if (n_tiles)
+            kron_fill_kernel<uint32_t><<<fill_grid, 256, 0, s>>>(
+                o, outer_c, nnz, n_tiles, (const uint32_t*)c->d_indptr, c->d_indices, c->d_data);
+    } else {
+        kron_indptr_kernel<uint64_t><<<grid_for(ctx, outer_c + 1), 256, 0, s>>>(
+            o, outer_c, nnz, (uint64_t*)c->d_indptr);
+        if (n_tiles)
+            kron_fill_kernel<uint64_t><<<fill_grid, 256, 0, s>>>(
+                o, outer_c, nnz, n_tiles, (const uint64_t*)c->d_indptr, c->d_indices, c->d_data);
     }
-    if (owned) sprs_b200_csmat_free(owned);
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(c);
-        return st;
-    }
-    *out = c;
-    return SPRS_B200_OK;
+    ctx->launches += n_tiles ? 2 : 1;
+    if (cudaGetLastError() != cudaSuccess) SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "kron: launch failed");
+    return finish_result(ctx, c, s, "kron", false, out);
 }
 
 int sprs_b200_csmat_transpose_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m,
@@ -496,30 +454,12 @@ int sprs_b200_csmat_transpose_view(sprs_b200_ctx* ctx, const sprs_b200_csmat* m,
     if (!ctx || !m || !out) return SPRS_B200_ERR_ARGUMENT;
     *out = nullptr;
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
-    auto* t = new sprs_b200_csmat();
-    t->ctx = ctx;
-    t->storage = m->storage == SPRS_B200_CSR ? SPRS_B200_CSC : SPRS_B200_CSR;
-    t->rows = m->cols;
-    t->cols = m->rows;
-    t->outer = m->outer;
-    t->inner = m->inner;
-    t->nnz = m->nnz;
-    t->indptr_bytes = m->indptr_bytes;
+    CsmatPtr t = new_result(ctx, m->storage == SPRS_B200_CSR ? SPRS_B200_CSC : SPRS_B200_CSR,
+                            m->cols, m->rows, m->nnz, m->indptr_bytes, Arrays::borrowed);
     t->d_indptr = m->d_indptr;
     t->d_indices = m->d_indices;
     t->d_data = m->d_data;
-    t->owns = false;
-    int st = spmv_prepare(ctx, t, ctx->stream, false);
-    if (st == SPRS_B200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-        sprs_b200_set_error(ctx, "transpose_view: partition kernel failed");
-        st = SPRS_B200_ERR_CUDA;
-    }
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(t);
-        return st;
-    }
-    *out = t;
-    return SPRS_B200_OK;
+    return finish_result(ctx, t, ctx->stream, "transpose_view", false, out);
 }
 
 }  // extern "C"

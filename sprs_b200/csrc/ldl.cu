@@ -54,19 +54,19 @@ struct sprs_b200_ldl {
     // symbolic: the input's pattern (copies), the permutation, L's structure
     uint64_t a_nnz = 0, a_outer = 0;
     int a_ipb = 4;
-    void* d_a_ip = nullptr;
-    uint32_t* d_a_idx = nullptr;
-    uint32_t *d_perm = nullptr, *d_pinv = nullptr;
-    uint32_t *d_colptr = nullptr, *d_lidx = nullptr;   // CSC of L
-    uint32_t *d_rowptr = nullptr, *d_cidx = nullptr;   // CSR of L's pattern
-    uint32_t *d_pat_pos = nullptr, *d_pat_slot = nullptr;  // per pattern entry, pattern order
+    Owned<void> d_a_ip;
+    Owned<uint32_t> d_a_idx;
+    Owned<uint32_t> d_perm, d_pinv;
+    Owned<uint32_t> d_colptr, d_lidx;       // CSC of L
+    Owned<uint32_t> d_rowptr, d_cidx;       // CSR of L's pattern
+    Owned<uint32_t> d_pat_pos, d_pat_slot;  // per pattern entry, pattern order
     // numeric
-    double *d_lcsr = nullptr, *d_lcsc = nullptr, *d_diag = nullptr, *d_tmp = nullptr;
-    uint32_t* d_flags = nullptr;
-    unsigned long long* d_words = nullptr;     // [0] ticket counter, [1] first singular row
-    unsigned long long* d_progress = nullptr;  // per warp of the launch
+    Owned<double> d_lcsr, d_lcsc, d_diag, d_tmp;
+    Owned<uint32_t> d_flags;
+    Owned<unsigned long long> d_words;     // [0] ticket counter, [1] first singular row
+    Owned<unsigned long long> d_progress;  // per warp of the launch
     uint64_t n_progress = 0;
-    unsigned long long* h_err = nullptr;       // pinned: a wait bound was exceeded
+    Owned<unsigned long long> h_err;       // pinned: a wait bound was exceeded
     cudaEvent_t ev_last = nullptr;
     uint32_t epoch = 0;
     int state = 0;  // numeric: 0 factor valid, 1 singular (sing_index), 2 no valid factor
@@ -258,8 +258,8 @@ unsigned blocks_for(uint64_t n, unsigned threads) {
 }
 
 template <typename T>
-int upload(sprs_b200_ctx* ctx, const std::vector<T>& h, T** d) {
-    SPRS_CUDA(ctx, cudaMalloc((void**)d, h.size() * sizeof(T) + 16));
+int upload(sprs_b200_ctx* ctx, const std::vector<T>& h, Owned<T>* d) {
+    SPRS_TRY(d->alloc(ctx, h.size() * sizeof(T) + 16, "ldl symbolic"));
     if (!h.empty())
         SPRS_CUDA(ctx, cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
     return SPRS_B200_OK;
@@ -366,16 +366,10 @@ void free_ldl(sprs_b200_ldl* h) {
     if (h->ctx) cudaSetDevice(h->ctx->device);
     if (h->plan_l) sprs_b200_trisolve_free(h->plan_l);
     if (h->plan_lt) sprs_b200_trisolve_free(h->plan_lt);
-    for (void* p : {(void*)h->d_a_ip, (void*)h->d_a_idx, (void*)h->d_perm, (void*)h->d_pinv,
-                    (void*)h->d_colptr, (void*)h->d_lidx, (void*)h->d_rowptr, (void*)h->d_cidx,
-                    (void*)h->d_pat_pos, (void*)h->d_pat_slot, (void*)h->d_lcsr, (void*)h->d_lcsc,
-                    (void*)h->d_diag, (void*)h->d_tmp, (void*)h->d_flags, (void*)h->d_words,
-                    (void*)h->d_progress})
-        if (p) cudaFree(p);
-    if (h->h_err) cudaFreeHost(h->h_err);
     if (h->ev_last) cudaEventDestroy(h->ev_last);
     delete h;
 }
+using LdlPtr = std::unique_ptr<sprs_b200_ldl, FreeWith<free_ldl>>;
 
 template <typename P>
 int build_symbolic(sprs_b200_ldl* h, const sprs_b200_csmat* m, const std::vector<uint32_t>& perm) {
@@ -404,8 +398,8 @@ int build_symbolic(sprs_b200_ldl* h, const sprs_b200_csmat* m, const std::vector
     h->a_nnz = m->nnz;
     h->a_outer = m->outer;
     h->a_ipb = m->indptr_bytes;
-    SPRS_CUDA(ctx, cudaMalloc(&h->d_a_ip, ip.size() * sizeof(P)));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&h->d_a_idx, m->nnz * sizeof(uint32_t) + 16));
+    SPRS_TRY(h->d_a_ip.alloc(ctx, ip.size() * sizeof(P), "ldl symbolic"));
+    SPRS_TRY(h->d_a_idx.alloc(ctx, m->nnz * sizeof(uint32_t) + 16, "ldl symbolic"));
     SPRS_CUDA(ctx, cudaMemcpy(h->d_a_ip, ip.data(), ip.size() * sizeof(P), cudaMemcpyHostToDevice));
     if (m->nnz)
         SPRS_CUDA(ctx, cudaMemcpy(h->d_a_idx, idx.data(), m->nnz * sizeof(uint32_t),
@@ -417,27 +411,21 @@ int alloc_numeric(sprs_b200_ldl* h) {
     sprs_b200_ctx* ctx = h->ctx;
     const sprs_b200_ldl* sy = h->sym;
     const uint64_t n = h->n, nnz = h->nnz_l;
-    SPRS_CUDA(ctx, cudaMalloc((void**)&h->d_lcsr, nnz * sizeof(double) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&h->d_lcsc, nnz * sizeof(double) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&h->d_diag, n * sizeof(double) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&h->d_tmp, n * sizeof(double) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&h->d_flags, n * sizeof(uint32_t) + 16));
+    SPRS_TRY(h->d_lcsr.alloc(ctx, nnz * sizeof(double) + 16, "ldl factor"));
+    SPRS_TRY(h->d_lcsc.alloc(ctx, nnz * sizeof(double) + 16, "ldl factor"));
+    SPRS_TRY(h->d_diag.alloc(ctx, n * sizeof(double) + 16, "ldl factor"));
+    SPRS_TRY(h->d_tmp.alloc(ctx, n * sizeof(double) + 16, "ldl factor"));
+    SPRS_TRY(h->d_flags.alloc(ctx, n * sizeof(uint32_t) + 16, "ldl factor"));
     SPRS_CUDA(ctx, cudaMemset(h->d_flags, 0, n * sizeof(uint32_t) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&h->d_words, 2 * sizeof(unsigned long long)));
+    SPRS_TRY(h->d_words.alloc(ctx, 2 * sizeof(unsigned long long), "ldl factor"));
     h->n_progress = (uint64_t)ctx->sm_count * LDL_CTAS_PER_SM * (LDL_THREADS / 32);
-    SPRS_CUDA(ctx, cudaMalloc((void**)&h->d_progress, h->n_progress * sizeof(unsigned long long)));
-    SPRS_CUDA(ctx, cudaMallocHost((void**)&h->h_err, sizeof(unsigned long long)));
+    SPRS_TRY(h->d_progress.alloc(ctx, h->n_progress * sizeof(unsigned long long), "ldl factor"));
+    SPRS_TRY(h->h_err.alloc_pinned(ctx, sizeof(unsigned long long), "ldl factor"));
     *h->h_err = 0;
     SPRS_CUDA(ctx, cudaEventCreateWithFlags(&h->ev_last, cudaEventDisableTiming));
     // L (CSR, unit lower) and L^T (the CSC arrays read as CSR, unit upper) for the solves
-    for (sprs_b200_csmat* v : {&h->l_csr, &h->lt_csr}) {
-        v->ctx = ctx;
-        v->storage = SPRS_B200_CSR;
-        v->rows = v->cols = v->outer = v->inner = n;
-        v->nnz = nnz;
-        v->indptr_bytes = 4;
-        v->owns = false;
-    }
+    h->l_csr = csmat_init(ctx, SPRS_B200_CSR, n, n, nnz, 4, Arrays::borrowed);
+    h->lt_csr = csmat_init(ctx, SPRS_B200_CSR, n, n, nnz, 4, Arrays::borrowed);
     h->l_csr.d_indptr = sy->d_rowptr;
     h->l_csr.d_indices = sy->d_cidx;
     h->l_csr.d_data = h->d_lcsr;
@@ -627,16 +615,12 @@ int sprs_b200_ldl_symbolic(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, const
     } else {
         for (uint64_t i = 0; i < n; ++i) p[i] = (uint32_t)i;
     }
-    auto* h = new sprs_b200_ldl();
+    LdlPtr h(new sprs_b200_ldl());
     h->ctx = ctx;
     h->n = n;
-    const int st = mat->indptr_bytes == 4 ? build_symbolic<uint32_t>(h, mat, p)
-                                          : build_symbolic<uint64_t>(h, mat, p);
-    if (st != SPRS_B200_OK) {
-        free_ldl(h);
-        return st;
-    }
-    *out = h;
+    SPRS_TRY(mat->indptr_bytes == 4 ? build_symbolic<uint32_t>(h.get(), mat, p)
+                                    : build_symbolic<uint64_t>(h.get(), mat, p));
+    *out = h.release();
     return SPRS_B200_OK;
 }
 
@@ -649,19 +633,16 @@ int sprs_b200_ldl_factor(const sprs_b200_ldl* sym, const sprs_b200_csmat* mat, s
     *out = nullptr;
     sprs_b200_ctx* ctx = sym->ctx;
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
-    auto* h = new sprs_b200_ldl();
+    LdlPtr h(new sprs_b200_ldl());
     h->ctx = ctx;
     h->sym = sym;
     h->n = sym->n;
     h->nnz_l = sym->nnz_l;
     h->state = 2;
-    int st = alloc_numeric(h);
-    if (st == SPRS_B200_OK) st = numeric(h, mat);
-    if (st != SPRS_B200_OK && st != SPRS_B200_ERR_SINGULAR) {
-        free_ldl(h);
-        return st;
-    }
-    *out = h;
+    SPRS_TRY(alloc_numeric(h.get()));
+    const int st = numeric(h.get(), mat);
+    if (st != SPRS_B200_OK && st != SPRS_B200_ERR_SINGULAR) return st;
+    *out = h.release();
     return st;
 }
 

@@ -233,12 +233,12 @@ struct sprs_b200_bicgstab {
     sprs_b200_matvec_fn op = nullptr;
     void* op_user = nullptr;
     uint64_t n = 0;
-    double* d_block = nullptr;  // one allocation: 8 vectors of `pitch` doubles
+    Owned<double> d_block;      // one allocation: 8 vectors of `pitch` doubles
     uint64_t pitch = 0;
     double *d_b = nullptr, *d_x = nullptr, *d_r = nullptr, *d_rhat = nullptr, *d_p = nullptr,
            *d_v = nullptr, *d_s = nullptr, *d_t = nullptr;
-    double* d_partials = nullptr;  // 2 * RED_MAX_BLOCKS, then the 2 results
-    double* h_result = nullptr;    // pinned, 2 doubles
+    Owned<double> d_partials;      // 2 * RED_MAX_BLOCKS, then the 2 results
+    Owned<double> h_result;        // pinned, 2 doubles
     int grid = 1;
     // bicgstab.rs:97-116
     uint64_t iteration_count = 0, soft_restart_count = 0, hard_restart_count = 0;
@@ -307,50 +307,33 @@ int create_common(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, sprs_b200_matv
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
     const sprs_b200_csmat* csr = nullptr;
     if (mat) SPRS_TRY(csmat_csr_view(ctx, mat, &csr));
-    auto* s = new sprs_b200_bicgstab();
+    std::unique_ptr<sprs_b200_bicgstab, FreeWith<sprs_b200_bicgstab_free>> s(
+        new sprs_b200_bicgstab());
     s->ctx = ctx;
     s->csr = csr;
     s->op = mat ? nullptr : op;
     s->op_user = op_user;
     s->n = n;
     s->pitch = (n + 31) / 32 * 32 + 32;  // 256-byte aligned vectors
-    int st = SPRS_B200_OK;
-    do {
-        cudaError_t e = cudaMalloc((void**)&s->d_block, 8 * s->pitch * sizeof(double));
-        if (e == cudaSuccess)
-            e = cudaMalloc((void**)&s->d_partials, (2 * RED_MAX_BLOCKS + 2) * sizeof(double));
-        if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_result, 2 * sizeof(double));
-        if (e != cudaSuccess) {
-            sprs_b200_set_error(ctx, cudaGetErrorString(e));
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        double** slots[8] = {&s->d_b, &s->d_x, &s->d_r, &s->d_rhat,
-                             &s->d_p, &s->d_v, &s->d_s, &s->d_t};
-        for (int i = 0; i < 8; ++i) *slots[i] = s->d_block + (uint64_t)i * s->pitch;
-        uint64_t blocks = (n + 4 * RED_THREADS - 1) / (4 * RED_THREADS);
-        if (blocks < 1) blocks = 1;
-        const uint64_t cap = (uint64_t)ctx->sm_count * 4 < RED_MAX_BLOCKS
-                                 ? (uint64_t)ctx->sm_count * 4
-                                 : RED_MAX_BLOCKS;
-        s->grid = (int)(blocks < cap ? blocks : cap);
-        if (n) {
-            cudaStream_t cs = ctx->stream;
-            e = cudaMemcpyAsync(s->d_x, x0, n * sizeof(double), kind, cs);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_b, b, n * sizeof(double), kind, cs);
-            if (e != cudaSuccess) {
-                sprs_b200_set_error(ctx, cudaGetErrorString(e));
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-        }
-        st = recompute_residual(s);  // synchronises the stream: x0 / b may be reused after
-    } while (0);
-    if (st != SPRS_B200_OK) {
-        sprs_b200_bicgstab_free(s);
-        return st;
+    SPRS_TRY(s->d_block.alloc(ctx, 8 * s->pitch * sizeof(double), "bicgstab"));
+    SPRS_TRY(s->d_partials.alloc(ctx, (2 * RED_MAX_BLOCKS + 2) * sizeof(double), "bicgstab"));
+    SPRS_TRY(s->h_result.alloc_pinned(ctx, 2 * sizeof(double), "bicgstab"));
+    double** slots[8] = {&s->d_b, &s->d_x, &s->d_r, &s->d_rhat,
+                         &s->d_p, &s->d_v, &s->d_s, &s->d_t};
+    for (int i = 0; i < 8; ++i) *slots[i] = s->d_block + (uint64_t)i * s->pitch;
+    uint64_t blocks = (n + 4 * RED_THREADS - 1) / (4 * RED_THREADS);
+    if (blocks < 1) blocks = 1;
+    const uint64_t cap = (uint64_t)ctx->sm_count * 4 < RED_MAX_BLOCKS
+                             ? (uint64_t)ctx->sm_count * 4
+                             : RED_MAX_BLOCKS;
+    s->grid = (int)(blocks < cap ? blocks : cap);
+    if (n) {
+        cudaStream_t cs = ctx->stream;
+        SPRS_CUDA(ctx, cudaMemcpyAsync(s->d_x, x0, n * sizeof(double), kind, cs));
+        SPRS_CUDA(ctx, cudaMemcpyAsync(s->d_b, b, n * sizeof(double), kind, cs));
     }
-    *out = s;
+    SPRS_TRY(recompute_residual(s.get()));  // synchronises the stream: x0 / b may be reused after
+    *out = s.release();
     return SPRS_B200_OK;
 }
 
@@ -378,9 +361,6 @@ int sprs_b200_bicgstab_new_op(sprs_b200_ctx* ctx, uint64_t n, sprs_b200_matvec_f
 int sprs_b200_bicgstab_free(sprs_b200_bicgstab* s) {
     if (!s) return SPRS_B200_OK;
     if (s->ctx) cudaSetDevice(s->ctx->device);
-    if (s->d_block) cudaFree(s->d_block);
-    if (s->d_partials) cudaFree(s->d_partials);
-    if (s->h_result) cudaFreeHost(s->h_result);
     delete s;
     return SPRS_B200_OK;
 }

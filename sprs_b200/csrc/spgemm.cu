@@ -47,11 +47,12 @@ struct sprs_b200_spgemm {
     const sprs_b200_csmat* a = nullptr;  // borrowed: must outlive the plan
     const sprs_b200_csmat* b = nullptr;
     uint64_t rows = 0, cols = 0, nnz_c = 0, n_prod = 0;
-    uint64_t* d_nprod = nullptr;  // [rows]
-    uint32_t* d_cnt = nullptr;    // [rows] nnz(C_i)
-    uint64_t* d_cptr = nullptr;   // [rows+1]
-    uint32_t* d_lists = nullptr;  // [3*rows] row lists per bin
-    uint32_t* d_counters = nullptr;  // [8]
+    // (stream-ordered allocations on the ctx stream: the pool keeps the memory across calls)
+    Owned<uint64_t> d_nprod;      // [rows]
+    Owned<uint32_t> d_cnt;        // [rows] nnz(C_i)
+    Owned<uint64_t> d_cptr;       // [rows+1]
+    Owned<uint32_t> d_lists;      // [3*rows] row lists per bin
+    Owned<uint32_t> d_counters;   // [8]
 };
 
 namespace {
@@ -827,19 +828,12 @@ int check_operands(sprs_b200_ctx* ctx, const sprs_b200_csmat* a, const sprs_b200
 }
 
 struct LargeWorkspace {
-    uint32_t* bitmaps = nullptr;
-    double* acc = nullptr;
+    Owned<uint32_t> bitmaps;
+    Owned<double> acc;
     unsigned grid = 0;
     size_t smem = 0;
     uint32_t words = 0;
 };
-
-void free_large(LargeWorkspace& w) {
-    if (w.bitmaps) cudaFree(w.bitmaps);
-    if (w.acc) cudaFree(w.acc);
-    w.bitmaps = nullptr;
-    w.acc = nullptr;
-}
 
 // bitmap placement (+ dense accumulators when need_acc) for the large-row kernels
 int plan_large(sprs_b200_ctx* ctx, uint64_t cols, uint32_t n_large, bool need_acc,
@@ -855,10 +849,9 @@ int plan_large(sprs_b200_ctx* ctx, uint64_t cols, uint32_t n_large, bool need_ac
     w->grid = grid;
     const bool smem_bitmap = cols <= BITMAP_SMEM_MAX_COLS;
     w->smem = smem_bitmap ? (size_t)w->words * 4 : 0;
-    if (!smem_bitmap)
-        SPRS_CUDA(ctx, cudaMalloc((void**)&w->bitmaps, (size_t)grid * w->words * 4));
+    if (!smem_bitmap) SPRS_TRY(w->bitmaps.alloc(ctx, (size_t)grid * w->words * 4, "spgemm"));
     if (need_acc) {
-        SPRS_CUDA(ctx, cudaMalloc((void**)&w->acc, (size_t)grid * cols * sizeof(double)));
+        SPRS_TRY(w->acc.alloc(ctx, (size_t)grid * cols * sizeof(double), "spgemm"));
         SPRS_CUDA(ctx, cudaMemsetAsync(w->acc, 0, (size_t)grid * cols * sizeof(double), s));
     }
     return SPRS_B200_OK;
@@ -905,8 +898,8 @@ int run_numeric(sprs_b200_ctx* ctx, sprs_b200_spgemm* p, uint32_t* d_cidx, doubl
     if (h_cnt[2]) {
         // lists[0 .. rows) and [rows .. 2 rows) are free again once small / medium have been
         // LAUNCHED?  No -- they are still being read; use fresh scratch for the split lists.
-        uint32_t* split = nullptr;
-        SPRS_CUDA(ctx, cudaMallocAsync((void**)&split, 2ull * h_cnt[2] * sizeof(uint32_t), s));
+        Owned<uint32_t> split;
+        SPRS_TRY(split.alloc_async(ctx, 2ull * h_cnt[2] * sizeof(uint32_t), s, "spgemm numeric"));
         uint32_t *panel_list = split, *hub_list = split + h_cnt[2];
         split_large_kernel<<<grid_for(h_cnt[2]), 256, 0, s>>>(a_ip, l2, h_cnt[2], PANEL_MAX_A,
                                                              panel_list, hub_list, p->d_counters);
@@ -945,10 +938,8 @@ int run_numeric(sprs_b200_ctx* ctx, sprs_b200_spgemm* p, uint32_t* d_cidx, doubl
                 ctx->launches += 1;
                 if (cudaStreamSynchronize(s) != cudaSuccess) st = SPRS_B200_ERR_CUDA;
             }
-            free_large(w);
         }
         if (cudaStreamSynchronize(s) != cudaSuccess) st = SPRS_B200_ERR_CUDA;
-        cudaFreeAsync(split, s);
         if (st != SPRS_B200_OK) SPRS_FAIL(ctx, st, "spgemm numeric (large rows) failed");
     }
     SPRS_CUDA(ctx, cudaGetLastError());
@@ -968,33 +959,26 @@ int sprs_b200_spgemm_symbolic(sprs_b200_ctx* ctx, const sprs_b200_csmat* a,
     SPRS_TRY(check_operands(ctx, a, b));
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
-    auto* p = new sprs_b200_spgemm();
+    std::unique_ptr<sprs_b200_spgemm, FreeWith<sprs_b200_spgemm_free>> p(new sprs_b200_spgemm());
     p->ctx = ctx;
     p->a = a;
     p->b = b;
     p->rows = a->rows;
     p->cols = b->cols;
     const uint32_t rows = (uint32_t)p->rows;
-    int st = SPRS_B200_OK;
-    do {
-        // (stream-ordered allocations: the pool keeps the memory across calls, api.cu)
-        if (cudaMallocAsync((void**)&p->d_nprod, (p->rows + 1) * 8, s) != cudaSuccess ||
-            cudaMallocAsync((void**)&p->d_cnt, (p->rows + 1) * 4, s) != cudaSuccess ||
-            cudaMallocAsync((void**)&p->d_cptr, (p->rows + 1) * 8, s) != cudaSuccess ||
-            cudaMallocAsync((void**)&p->d_lists, (3 * p->rows + 1) * 4, s) != cudaSuccess ||
-            cudaMallocAsync((void**)&p->d_counters, 8 * 4, s) != cudaSuccess) {
-            sprs_b200_set_error(ctx, "spgemm: cudaMalloc failed");
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        cudaMemsetAsync(p->d_cptr, 0, (p->rows + 1) * 8, s);
-        if (rows == 0) break;
+    SPRS_TRY(p->d_nprod.alloc_async(ctx, (p->rows + 1) * 8, s, "spgemm symbolic"));
+    SPRS_TRY(p->d_cnt.alloc_async(ctx, (p->rows + 1) * 4, s, "spgemm symbolic"));
+    SPRS_TRY(p->d_cptr.alloc_async(ctx, (p->rows + 1) * 8, s, "spgemm symbolic"));
+    SPRS_TRY(p->d_lists.alloc_async(ctx, (3 * p->rows + 1) * 4, s, "spgemm symbolic"));
+    SPRS_TRY(p->d_counters.alloc_async(ctx, 8 * 4, s, "spgemm symbolic"));
+    cudaMemsetAsync(p->d_cptr, 0, (p->rows + 1) * 8, s);
+    if (rows) {
         const uint32_t *a_ip = (const uint32_t*)a->d_indptr, *b_ip = (const uint32_t*)b->d_indptr;
         const unsigned cap = (unsigned)ctx->sm_count * 8;
         nprod_kernel<<<std::min<unsigned>((rows + WARPS - 1) / WARPS, cap * 4), NT, 0, s>>>(
             a_ip, a->d_indices, b_ip, rows, p->d_nprod);
         cudaMemsetAsync(p->d_counters, 0, 8 * sizeof(uint32_t), s);
-            // with the bitmap in shared memory (no probing, fixed cost ~ cols / 32 words) the
+        // with the bitmap in shared memory (no probing, fixed cost ~ cols / 32 words) the
         // hash set only pays below ~cols/256 products
         uint32_t sym_m_max = SYM_M_MAX;
         if (p->cols <= BITMAP_SMEM_MAX_COLS)
@@ -1005,11 +989,8 @@ int sprs_b200_spgemm_symbolic(sprs_b200_ctx* ctx, const sprs_b200_csmat* a,
         uint32_t h_cnt[8];
         if (cudaMemcpyAsync(h_cnt, p->d_counters, sizeof(h_cnt), cudaMemcpyDeviceToHost, s) !=
                 cudaSuccess ||
-            cudaStreamSynchronize(s) != cudaSuccess) {
-            sprs_b200_set_error(ctx, "spgemm symbolic: binning failed");
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
+            cudaStreamSynchronize(s) != cudaSuccess)
+            SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "spgemm symbolic: binning failed");
         const uint32_t *l0 = p->d_lists, *l1 = p->d_lists + rows, *l2 = p->d_lists + 2ull * rows;
         if (h_cnt[0]) {
             sym_small_kernel<<<std::min<unsigned>((h_cnt[0] + WARPS - 1) / WARPS, cap * 4), NT, 0,
@@ -1028,7 +1009,7 @@ int sprs_b200_spgemm_symbolic(sprs_b200_ctx* ctx, const sprs_b200_csmat* a,
         }
         if (h_cnt[2]) {
             LargeWorkspace w;
-            if ((st = plan_large(ctx, p->cols, h_cnt[2], false, &w, s)) != SPRS_B200_OK) break;
+            SPRS_TRY(plan_large(ctx, p->cols, h_cnt[2], false, &w, s));
             auto kern = w.smem ? sym_large_kernel<true> : sym_large_kernel<false>;
             if (w.smem)
                 cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1038,26 +1019,17 @@ int sprs_b200_spgemm_symbolic(sprs_b200_ctx* ctx, const sprs_b200_csmat* a,
                                                   p->d_counters + 5);
             ctx->launches += 1;
             cudaStreamSynchronize(s);
-            free_large(w);
         }
-        if ((st = device_exclusive_scan<uint32_t, uint64_t>(ctx, p->d_cnt, rows, p->d_cptr, s)) !=
-            SPRS_B200_OK)
-            break;
+        SPRS_TRY((device_exclusive_scan<uint32_t, uint64_t>(ctx, p->d_cnt, rows, p->d_cptr, s)));
         // n_prod total: scan of per-row n_prod would need another buffer; reduce on the host
         // side of the plan lazily (sprs_b200_spgemm_nprod)
         if (cudaMemcpyAsync(&p->nnz_c, p->d_cptr + rows, 8, cudaMemcpyDeviceToHost, s) !=
                 cudaSuccess ||
-            cudaStreamSynchronize(s) != cudaSuccess || cudaGetLastError() != cudaSuccess) {
-            sprs_b200_set_error(ctx, "spgemm symbolic: kernel failed");
-            st = SPRS_B200_ERR_CUDA;
-        }
-    } while (0);
-    if (st != SPRS_B200_OK) {
-        sprs_b200_spgemm_free(p);
-        return st;
+            cudaStreamSynchronize(s) != cudaSuccess || cudaGetLastError() != cudaSuccess)
+            SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "spgemm symbolic: kernel failed");
     }
-    *plan = p;
     *nnz_c = p->nnz_c;
+    *plan = p.release();
     return SPRS_B200_OK;
 }
 
@@ -1066,47 +1038,21 @@ int sprs_b200_spgemm_numeric_dev(sprs_b200_ctx* ctx, sprs_b200_spgemm* p, sprs_b
     *c = nullptr;
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
-    auto* m = new sprs_b200_csmat();
-    m->ctx = ctx;
-    m->storage = SPRS_B200_CSR;
-    m->rows = p->rows;
-    m->cols = p->cols;
-    m->nnz = p->nnz_c;
-    m->outer = p->rows;
-    m->inner = p->cols;
-    m->indptr_bytes = p->nnz_c >= 0xffffffffull ? 8 : 4;
-    m->pooled = true;
-    int st = SPRS_B200_OK;
-    do {
-        if (cudaMallocAsync(&m->d_indptr, (m->rows + 1) * (size_t)m->indptr_bytes + 16, s) != cudaSuccess ||
-            cudaMallocAsync((void**)&m->d_indices, m->nnz * 4 + 16, s) != cudaSuccess ||
-            cudaMallocAsync((void**)&m->d_data, m->nnz * 8 + 16, s) != cudaSuccess) {
-            sprs_b200_set_error(ctx, "spgemm numeric: cudaMalloc of C failed");
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        if (m->indptr_bytes == 4) {
-            widen_kernel<uint64_t, uint32_t><<<grid_for(m->rows + 1), 256, 0, s>>>(
-                p->d_cptr, (uint32_t*)m->d_indptr, m->rows + 1);
-            ctx->launches += 1;
-        } else {
-            cudaMemcpyAsync(m->d_indptr, p->d_cptr, (m->rows + 1) * 8, cudaMemcpyDeviceToDevice, s);
-        }
-        if ((st = run_numeric(ctx, p, m->d_indices, m->d_data, s)) != SPRS_B200_OK) break;
-        // (no SpMV hot set for a product: its build would run inside every SpGEMM call and
-        // would need 4 more bytes per non-zero next to a result that may fill the device)
-        if ((st = spmv_prepare(ctx, m, s, false)) != SPRS_B200_OK) break;
-        if (cudaStreamSynchronize(s) != cudaSuccess || cudaGetLastError() != cudaSuccess) {
-            sprs_b200_set_error(ctx, "spgemm numeric: kernel failed");
-            st = SPRS_B200_ERR_CUDA;
-        }
-    } while (0);
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(m);
-        return st;
+    // (the SPRS_B200_FORCE_INDPTR64 test hook of indptr_bytes_for does not apply to products)
+    CsmatPtr m = new_result(ctx, SPRS_B200_CSR, p->rows, p->cols, p->nnz_c,
+                            p->nnz_c >= 0xffffffffull ? 8 : 4, Arrays::pooled);
+    SPRS_TRY(alloc_result(ctx, m.get(), s, "spgemm numeric"));
+    if (m->indptr_bytes == 4) {
+        widen_kernel<uint64_t, uint32_t><<<grid_for(m->rows + 1), 256, 0, s>>>(
+            p->d_cptr, (uint32_t*)m->d_indptr, m->rows + 1);
+        ctx->launches += 1;
+    } else {
+        cudaMemcpyAsync(m->d_indptr, p->d_cptr, (m->rows + 1) * 8, cudaMemcpyDeviceToDevice, s);
     }
-    *c = m;
-    return SPRS_B200_OK;
+    SPRS_TRY(run_numeric(ctx, p, m->d_indices, m->d_data, s));
+    // (no SpMV hot set for a product: its build would run inside every SpGEMM call and
+    // would need 4 more bytes per non-zero next to a result that may fill the device)
+    return finish_result(ctx, m, s, "spgemm numeric", false, c);
 }
 
 int sprs_b200_spgemm_numeric(sprs_b200_ctx* ctx, sprs_b200_spgemm* p, void* c_indptr,
@@ -1137,12 +1083,6 @@ uint64_t sprs_b200_spgemm_nprod(const sprs_b200_spgemm* p) {
 int sprs_b200_spgemm_free(sprs_b200_spgemm* p) {
     if (!p) return SPRS_B200_OK;
     if (p->ctx) cudaSetDevice(p->ctx->device);
-    cudaStream_t s = p->ctx ? p->ctx->stream : nullptr;
-    if (p->d_nprod) cudaFreeAsync(p->d_nprod, s);
-    if (p->d_cnt) cudaFreeAsync(p->d_cnt, s);
-    if (p->d_cptr) cudaFreeAsync(p->d_cptr, s);
-    if (p->d_lists) cudaFreeAsync(p->d_lists, s);
-    if (p->d_counters) cudaFreeAsync(p->d_counters, s);
     delete p;
     return SPRS_B200_OK;
 }

@@ -702,89 +702,76 @@ int spmv_prepare_hot(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s) {
     if (cfg.k == 0 || m->nnz == 0 || m->cols == 0 || m->cols >= HOT_TAG) return SPRS_B200_OK;
     if (!cfg.forced && m->nnz < SPMV_HOT_MIN_NNZ) return SPRS_B200_OK;
     const uint32_t cols = (uint32_t)m->cols;
-    uint32_t *counts = nullptr, *hist = nullptr, *slot = nullptr, *hot_col = nullptr,
-             *hot_idx = nullptr;
-    uint8_t* flag = nullptr;
-    unsigned long long* d_hot_nnz = nullptr;
     const unsigned grid_nnz =
         (unsigned)std::min<uint64_t>((m->nnz + 255) / 256, (uint64_t)ctx->sm_count * 16);
     const unsigned grid_cols = (unsigned)((cols + 255) / 256);
-    // returns with m->n_hot still 0 wherever the mirror gets no hot set
-    auto build = [&]() -> int {
-        if (cudaMalloc((void**)&counts, cols * sizeof(uint32_t)) != cudaSuccess ||
-            cudaMalloc((void**)&hist, 65536 * sizeof(uint32_t)) != cudaSuccess ||
-            cudaMalloc((void**)&flag, cols) != cudaSuccess ||
-            cudaMalloc((void**)&slot, (cols + 1ull) * sizeof(uint32_t)) != cudaSuccess ||
-            cudaMalloc((void**)&d_hot_nnz, sizeof(unsigned long long)) != cudaSuccess)
-            return SPRS_B200_OK;  // not enough memory for the build: no hot set
-        // ---- references per column, then the count of the K-th most referenced column
-        SPRS_CUDA(ctx, cudaMemsetAsync(counts, 0, cols * sizeof(uint32_t), s));
+    // (returns OK with m->n_hot still 0 wherever the mirror gets no hot set; a buffer that cannot
+    // be allocated means no hot set, not an error)
+    Owned<uint32_t> counts, hist, slot, hot_col, hot_idx;
+    Owned<uint8_t> flag;
+    Owned<unsigned long long> d_hot_nnz;
+    if (counts.alloc(ctx, cols * sizeof(uint32_t), "spmv hot set") != SPRS_B200_OK ||
+        hist.alloc(ctx, 65536 * sizeof(uint32_t), "spmv hot set") != SPRS_B200_OK ||
+        flag.alloc(ctx, cols, "spmv hot set") != SPRS_B200_OK ||
+        slot.alloc(ctx, (cols + 1ull) * sizeof(uint32_t), "spmv hot set") != SPRS_B200_OK ||
+        d_hot_nnz.alloc(ctx, sizeof(unsigned long long), "spmv hot set") != SPRS_B200_OK)
+        return SPRS_B200_OK;
+    // ---- references per column, then the count of the K-th most referenced column
+    SPRS_CUDA(ctx, cudaMemsetAsync(counts, 0, cols * sizeof(uint32_t), s));
+    SPRS_CUDA(ctx, cudaMemsetAsync(hist, 0, 65536 * sizeof(uint32_t), s));
+    SPRS_CUDA(ctx, cudaMemsetAsync(d_hot_nnz, 0, sizeof(unsigned long long), s));
+    hot_count_kernel<<<grid_nnz, 256, 0, s>>>(m->d_indices, m->nnz, counts);
+    hot_count_hist_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, ~0u, hist);
+    ctx->launches += 2;
+    std::vector<uint32_t> h(65536);
+    SPRS_CUDA(ctx, cudaMemcpyAsync(h.data(), hist, 65536 * sizeof(uint32_t),
+                                   cudaMemcpyDeviceToHost, s));
+    SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+    uint64_t above = 0, referenced = 0;
+    for (uint32_t b = 0; b < 65536; ++b) referenced += h[b];
+    uint32_t k = cfg.k, thr = 1, ties = 0xffffffffu;  // K or fewer referenced columns: all
+    if (referenced > k) {
+        uint32_t bhi = 65535;  // (the loops stop: the bins hold more than K columns)
+        while (above + h[bhi] < k) above += h[bhi--];
         SPRS_CUDA(ctx, cudaMemsetAsync(hist, 0, 65536 * sizeof(uint32_t), s));
-        SPRS_CUDA(ctx, cudaMemsetAsync(d_hot_nnz, 0, sizeof(unsigned long long), s));
-        hot_count_kernel<<<grid_nnz, 256, 0, s>>>(m->d_indices, m->nnz, counts);
-        hot_count_hist_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, ~0u, hist);
-        ctx->launches += 2;
-        std::vector<uint32_t> h(65536);
+        hot_count_hist_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, bhi, hist);
+        ctx->launches += 1;
         SPRS_CUDA(ctx, cudaMemcpyAsync(h.data(), hist, 65536 * sizeof(uint32_t),
                                        cudaMemcpyDeviceToHost, s));
         SPRS_CUDA(ctx, cudaStreamSynchronize(s));
-        uint64_t above = 0, referenced = 0;
-        for (uint32_t b = 0; b < 65536; ++b) referenced += h[b];
-        uint32_t k = cfg.k, thr = 1, ties = 0xffffffffu;  // K or fewer referenced columns: all
-        if (referenced > k) {
-            uint32_t bhi = 65535;  // (the loops stop: the bins hold more than K columns)
-            while (above + h[bhi] < k) above += h[bhi--];
-            SPRS_CUDA(ctx, cudaMemsetAsync(hist, 0, 65536 * sizeof(uint32_t), s));
-            hot_count_hist_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, bhi, hist);
-            ctx->launches += 1;
-            SPRS_CUDA(ctx, cudaMemcpyAsync(h.data(), hist, 65536 * sizeof(uint32_t),
-                                           cudaMemcpyDeviceToHost, s));
-            SPRS_CUDA(ctx, cudaStreamSynchronize(s));
-            uint32_t blo = 65535;
-            while (above + h[blo] < k) above += h[blo--];
-            thr = (bhi << 16) | blo;
-            ties = k - (uint32_t)above;  // columns of count thr to take, in column order
-        } else {
-            k = (uint32_t)referenced;
-        }
-        // ---- select, slots in column order, tag map
-        hot_flag_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, thr, nullptr, 0, flag);
-        ctx->launches += 1;
-        SPRS_TRY((device_exclusive_scan<uint8_t, uint32_t>(ctx, flag, cols, slot, s)));
-        hot_flag_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, thr, slot, ties, flag);
-        ctx->launches += 1;
-        SPRS_TRY((device_exclusive_scan<uint8_t, uint32_t>(ctx, flag, cols, slot, s)));
-        if (cudaMalloc((void**)&hot_col, k * sizeof(uint32_t)) != cudaSuccess) return SPRS_B200_OK;
-        hot_map_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, flag, slot, hot_col, d_hot_nnz);
-        ctx->launches += 1;
-        unsigned long long hot_nnz = 0;
-        SPRS_CUDA(ctx, cudaMemcpyAsync(&hot_nnz, d_hot_nnz, sizeof(hot_nnz), cudaMemcpyDeviceToHost, s));
-        SPRS_CUDA(ctx, cudaStreamSynchronize(s));
-        if (!cfg.forced && (double)hot_nnz < SPMV_HOT_MIN_SHARE * (double)m->nnz) return SPRS_B200_OK;
-        // ---- the tagged index stream (+4 bytes per non-zero)
-        if (cudaMalloc((void**)&hot_idx, m->nnz * sizeof(uint32_t) + 16) != cudaSuccess)
-            return SPRS_B200_OK;
-        hot_tag_kernel<<<grid_nnz, 256, 0, s>>>(m->d_indices, m->nnz, counts, hot_idx);
-        ctx->launches += 1;
-        SPRS_CUDA(ctx, cudaStreamSynchronize(s));
-        SPRS_CUDA(ctx, cudaGetLastError());
-        m->d_hot_col = hot_col;
-        m->d_hot_idx = hot_idx;
-        m->n_hot = k;
-        return SPRS_B200_OK;
-    };
-    const int st = build();
-    if (m->n_hot == 0) {
-        cudaGetLastError();  // (a failed allocation leaves an error behind: it is not one here)
-        if (hot_col) cudaFree(hot_col);
-        if (hot_idx) cudaFree(hot_idx);
+        uint32_t blo = 65535;
+        while (above + h[blo] < k) above += h[blo--];
+        thr = (bhi << 16) | blo;
+        ties = k - (uint32_t)above;  // columns of count thr to take, in column order
+    } else {
+        k = (uint32_t)referenced;
     }
-    if (counts) cudaFree(counts);
-    if (hist) cudaFree(hist);
-    if (flag) cudaFree(flag);
-    if (slot) cudaFree(slot);
-    if (d_hot_nnz) cudaFree(d_hot_nnz);
-    return st;
+    // ---- select, slots in column order, tag map
+    hot_flag_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, thr, nullptr, 0, flag);
+    ctx->launches += 1;
+    SPRS_TRY((device_exclusive_scan<uint8_t, uint32_t>(ctx, flag, cols, slot, s)));
+    hot_flag_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, thr, slot, ties, flag);
+    ctx->launches += 1;
+    SPRS_TRY((device_exclusive_scan<uint8_t, uint32_t>(ctx, flag, cols, slot, s)));
+    if (hot_col.alloc(ctx, k * sizeof(uint32_t), "spmv hot set") != SPRS_B200_OK)
+        return SPRS_B200_OK;
+    hot_map_kernel<<<grid_cols, 256, 0, s>>>(counts, cols, flag, slot, hot_col, d_hot_nnz);
+    ctx->launches += 1;
+    unsigned long long hot_nnz = 0;
+    SPRS_CUDA(ctx, cudaMemcpyAsync(&hot_nnz, d_hot_nnz, sizeof(hot_nnz), cudaMemcpyDeviceToHost, s));
+    SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+    if (!cfg.forced && (double)hot_nnz < SPMV_HOT_MIN_SHARE * (double)m->nnz) return SPRS_B200_OK;
+    // ---- the tagged index stream (+4 bytes per non-zero)
+    if (hot_idx.alloc(ctx, m->nnz * sizeof(uint32_t) + 16, "spmv hot set") != SPRS_B200_OK)
+        return SPRS_B200_OK;
+    hot_tag_kernel<<<grid_nnz, 256, 0, s>>>(m->d_indices, m->nnz, counts, hot_idx);
+    ctx->launches += 1;
+    SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+    SPRS_CUDA(ctx, cudaGetLastError());
+    m->d_hot_col = hot_col.release();
+    m->d_hot_idx = hot_idx.release();
+    m->n_hot = k;
+    return SPRS_B200_OK;
 }
 
 int check_spmv_args(sprs_b200_ctx* ctx, const sprs_b200_csmat* m) {
@@ -804,9 +791,12 @@ int spmv_prepare(sprs_b200_ctx* ctx, sprs_b200_csmat* m, cudaStream_t s, bool ho
     const uint32_t row_cost = (uint32_t)spmv_variant().row_cost;
     const uint64_t total = m->nnz + (uint64_t)row_cost * m->rows;
     m->n_tiles = total == 0 ? 1 : (total + w - 1) / w;
-    SPRS_CUDA(ctx, cudaMalloc((void**)&m->d_tile_row, (m->n_tiles + 1) * sizeof(uint32_t)));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&m->d_tile_k, (m->n_tiles + 1) * (size_t)m->indptr_bytes));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&m->d_carry, m->n_tiles * sizeof(double)));
+    SPRS_TRY(mem_alloc(ctx, MemKind::device, (m->n_tiles + 1) * sizeof(uint32_t), nullptr,
+                       "spmv partition", (void**)&m->d_tile_row));
+    SPRS_TRY(mem_alloc(ctx, MemKind::device, (m->n_tiles + 1) * (size_t)m->indptr_bytes, nullptr,
+                       "spmv partition", &m->d_tile_k));
+    SPRS_TRY(mem_alloc(ctx, MemKind::device, m->n_tiles * sizeof(double), nullptr,
+                       "spmv partition", (void**)&m->d_carry));
     const uint64_t n = m->n_tiles + 1;
     const unsigned grid = (unsigned)((n + 255) / 256);
     if (m->indptr_bytes == 4)

@@ -142,30 +142,18 @@ inline unsigned grid_for(uint64_t n) { return (unsigned)((n + 255) / 256); }
 // Stable LSD radix sort of n (key, pos) pairs on `key_bits` bits; pos_in == nullptr means
 // pos = 0..n-1.  Uses the caller's ping-pong buffers; returns pointers to the sorted arrays.
 struct SortBuffers {
-    uint32_t *kbuf[2] = {nullptr, nullptr}, *pbuf[2] = {nullptr, nullptr}, *hist = nullptr;
-    uint64_t* offs = nullptr;
+    Owned<uint32_t> kbuf[2], pbuf[2], hist;
+    Owned<uint64_t> offs;
     uint32_t nblocks = 0;
-    int alloc(uint64_t n) {
+    int alloc(sprs_b200_ctx* ctx, uint64_t n, const char* what) {
         nblocks = (uint32_t)((n + RS_CHUNK - 1) / RS_CHUNK);
-        if (cudaMalloc((void**)&kbuf[0], n * 4) != cudaSuccess ||
-            cudaMalloc((void**)&kbuf[1], n * 4) != cudaSuccess ||
-            cudaMalloc((void**)&pbuf[0], n * 4) != cudaSuccess ||
-            cudaMalloc((void**)&pbuf[1], n * 4) != cudaSuccess ||
-            cudaMalloc((void**)&hist, 256ull * nblocks * 4) != cudaSuccess ||
-            cudaMalloc((void**)&offs, (256ull * nblocks + 1) * 8) != cudaSuccess)
-            return SPRS_B200_ERR_CUDA;
-        return SPRS_B200_OK;
-    }
-    void release() {
         for (int i = 0; i < 2; ++i) {
-            if (kbuf[i]) cudaFree(kbuf[i]);
-            if (pbuf[i]) cudaFree(pbuf[i]);
-            kbuf[i] = pbuf[i] = nullptr;
+            SPRS_TRY(kbuf[i].alloc(ctx, n * 4, what));
+            SPRS_TRY(pbuf[i].alloc(ctx, n * 4, what));
         }
-        if (hist) cudaFree(hist);
-        if (offs) cudaFree(offs);
-        hist = nullptr;
-        offs = nullptr;
+        SPRS_TRY(hist.alloc(ctx, 256ull * nblocks * 4, what));
+        SPRS_TRY(offs.alloc(ctx, (256ull * nblocks + 1) * 8, what));
+        return SPRS_B200_OK;
     }
 };
 
@@ -231,8 +219,7 @@ __global__ void compress_runs_kernel(const uint32_t* __restrict__ row, const uin
 
 }  // namespace
 
-int transpose_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, sprs_b200_csmat* t,
-                     cudaStream_t s) {
+int transpose_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, CsmatPtr* out, cudaStream_t s) {
     if (m->nnz >= 0xffffffffull)
         SPRS_FAIL(ctx, SPRS_B200_ERR_UNSUPPORTED, "to_other_storage: nnz >= 2^32 not supported");
     // gh374 (sprs/tests/gh374.rs): the outer indices must fit the index type; device
@@ -240,51 +227,33 @@ int transpose_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, sprs_b200_csm
     if (m->outer > 0xffffffffull)
         SPRS_FAIL(ctx, SPRS_B200_ERR_INDEX_RANGE,
                   "Index type is not large enough to hold the number of rows requested");
-    t->ctx = ctx;
-    t->storage = m->storage == SPRS_B200_CSR ? SPRS_B200_CSC : SPRS_B200_CSR;
-    t->rows = m->rows;
-    t->cols = m->cols;
-    t->nnz = m->nnz;
-    t->outer = m->inner;
-    t->inner = m->outer;
-    t->indptr_bytes = 4;
-    t->owns = true;
+    CsmatPtr t = new_result(ctx, m->storage == SPRS_B200_CSR ? SPRS_B200_CSC : SPRS_B200_CSR,
+                            m->rows, m->cols, m->nnz, 4, Arrays::owned);
     const uint64_t nnz = m->nnz, inner = m->inner;
-    SPRS_CUDA(ctx, cudaMalloc(&t->d_indptr, (inner + 1) * sizeof(uint32_t) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&t->d_indices, nnz * sizeof(uint32_t) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&t->d_data, nnz * sizeof(double) + 16));
+    SPRS_TRY(alloc_result(ctx, t.get(), s, "to_other_storage"));
 
     // ---- new indptr: histogram of inner indices + exclusive scan
-    uint32_t* counts = nullptr;
-    uint64_t* ip64 = nullptr;
-    SPRS_CUDA(ctx, cudaMalloc((void**)&counts, (inner + 1) * sizeof(uint32_t)));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&ip64, (inner + 1) * sizeof(uint64_t)));
-    int st = SPRS_B200_OK;
-    SortBuffers sb;
-    do {
-        cudaError_t e = cudaMemsetAsync(counts, 0, (inner + 1) * sizeof(uint32_t), s);
-        if (e != cudaSuccess) { st = SPRS_B200_ERR_CUDA; break; }
-        if (nnz) {
-            count_inner_kernel<<<grid_for(nnz), 256, 0, s>>>(m->d_indices, nnz, counts);
-            ctx->launches += 1;
-        }
-        if ((st = device_exclusive_scan<uint32_t, uint64_t>(ctx, counts, inner, ip64, s)) !=
-            SPRS_B200_OK)
-            break;
-        narrow_kernel<uint64_t, uint32_t><<<grid_for(inner + 1), 256, 0, s>>>(
-            ip64, (uint32_t*)t->d_indptr, inner + 1);
+    Owned<uint32_t> counts;
+    Owned<uint64_t> ip64;
+    SPRS_TRY(counts.alloc(ctx, (inner + 1) * sizeof(uint32_t), "to_other_storage"));
+    SPRS_TRY(ip64.alloc(ctx, (inner + 1) * sizeof(uint64_t), "to_other_storage"));
+    SPRS_CUDA(ctx, cudaMemsetAsync(counts, 0, (inner + 1) * sizeof(uint32_t), s));
+    if (nnz) {
+        count_inner_kernel<<<grid_for(nnz), 256, 0, s>>>(m->d_indices, nnz, counts);
         ctx->launches += 1;
-        if (nnz == 0) break;
+    }
+    SPRS_TRY((device_exclusive_scan<uint32_t, uint64_t>(ctx, counts, inner, ip64, s)));
+    narrow_kernel<uint64_t, uint32_t><<<grid_for(inner + 1), 256, 0, s>>>(
+        ip64, (uint32_t*)t->d_indptr, inner + 1);
+    ctx->launches += 1;
 
-        // ---- stable LSD radix sort of (inner index, position)
-        if ((st = sb.alloc(nnz)) != SPRS_B200_OK) {
-            sprs_b200_set_error(ctx, "to_other_storage: cudaMalloc failed");
-            break;
-        }
+    // ---- stable LSD radix sort of (inner index, position)
+    SortBuffers sb;
+    if (nnz) {
+        SPRS_TRY(sb.alloc(ctx, nnz, "to_other_storage"));
         const uint32_t *kin = nullptr, *pin = nullptr;
-        if ((st = stable_sort_pairs(ctx, sb, m->d_indices, nullptr, nnz, bits_for(inner), s, &kin,
-                                    &pin)) != SPRS_B200_OK)
-            break;
+        SPRS_TRY(stable_sort_pairs(ctx, sb, m->d_indices, nullptr, nnz, bits_for(inner), s, &kin,
+                                   &pin));
         if (m->indptr_bytes == 4)
             gather_transposed_kernel<uint32_t><<<grid_for(nnz), 256, 0, s>>>(
                 pin, nnz, (const uint32_t*)m->d_indptr, (uint32_t)m->outer, m->d_data,
@@ -294,17 +263,11 @@ int transpose_launch(sprs_b200_ctx* ctx, const sprs_b200_csmat* m, sprs_b200_csm
                 pin, nnz, (const uint64_t*)m->d_indptr, (uint32_t)m->outer, m->d_data,
                 t->d_indices, t->d_data);
         ctx->launches += 1;
-    } while (0);
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (st == SPRS_B200_OK && e == cudaSuccess) e = cudaGetLastError();
-    if (st == SPRS_B200_OK && e != cudaSuccess) {
-        sprs_b200_set_error(ctx, cudaGetErrorString(e));
-        st = SPRS_B200_ERR_CUDA;
     }
-    cudaFree(counts);
-    cudaFree(ip64);
-    sb.release();
-    return st;
+    SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+    SPRS_CUDA(ctx, cudaGetLastError());
+    *out = std::move(t);
+    return SPRS_B200_OK;
 }
 
 // COO (device arrays, any order, duplicates allowed) -> CSR mirror with ascending unique
@@ -322,109 +285,65 @@ __global__ void triplet_bounds_kernel(const uint32_t* __restrict__ row, const ui
 
 int triplets_to_csr_launch(sprs_b200_ctx* ctx, uint64_t rows, uint64_t cols, uint64_t n,
                            const uint32_t* d_row, const uint32_t* d_col, const double* d_val,
-                           sprs_b200_csmat* t, cudaStream_t s) {
+                           CsmatPtr* out, cudaStream_t s) {
     if (n >= 0xffffffffull || rows > 0xffffffffull || cols > 0xffffffffull)
         SPRS_FAIL(ctx, SPRS_B200_ERR_INDEX_RANGE, "from_triplets: needs nnz, rows, cols < 2^32");
     if (n) {  // the reference panics on an out-of-range triplet (TriMatBase::add_triplet asserts);
               // here it would be an out-of-bounds device write in the counting pass
-        unsigned long long* d_bad = nullptr;
+        Owned<unsigned long long> d_bad;
         unsigned long long h_bad = 0;
-        SPRS_CUDA(ctx, cudaMalloc((void**)&d_bad, 8));
+        SPRS_TRY(d_bad.alloc(ctx, 8, "from_triplets"));
         cudaMemsetAsync(d_bad, 0, 8, s);
         triplet_bounds_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_row, d_col, n, (uint32_t)rows,
                                                                           (uint32_t)cols, d_bad);
         ctx->launches += 1;
         cudaMemcpyAsync(&h_bad, d_bad, 8, cudaMemcpyDeviceToHost, s);
         const cudaError_t e = cudaStreamSynchronize(s);
-        cudaFree(d_bad);
         if (e != cudaSuccess) SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "from_triplets: %s", cudaGetErrorString(e));
         if (h_bad)
             SPRS_FAIL(ctx, SPRS_B200_ERR_STRUCTURE, "from_triplets: %llu triplet(s) outside %llu x %llu",
                       h_bad, (unsigned long long)rows, (unsigned long long)cols);
     }
-    t->ctx = ctx;
-    t->storage = SPRS_B200_CSR;
-    t->rows = rows;
-    t->cols = cols;
-    t->outer = rows;
-    t->inner = cols;
-    t->indptr_bytes = 4;
-    t->owns = true;
-    t->nnz = 0;
-    SPRS_CUDA(ctx, cudaMalloc(&t->d_indptr, (rows + 1) * sizeof(uint32_t) + 16));
-    uint32_t *counts = nullptr, *row_s = nullptr, *col_s = nullptr, *flag = nullptr;
-    uint64_t *ip64 = nullptr, *uidx = nullptr;
+    Owned<uint32_t> counts, row_s, col_s, flag;
+    Owned<uint64_t> ip64, uidx;
     SortBuffers sb;
-    int st = SPRS_B200_OK;
-    do {
-        if (cudaMalloc((void**)&counts, (rows + 1) * 4) != cudaSuccess ||
-            cudaMalloc((void**)&ip64, (rows + 1) * 8) != cudaSuccess) {
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        cudaMemsetAsync(counts, 0, (rows + 1) * 4, s);
-        uint64_t n_unique = 0;
-        if (n) {
-            if (cudaMalloc((void**)&row_s, n * 4) != cudaSuccess ||
-                cudaMalloc((void**)&col_s, n * 4) != cudaSuccess ||
-                cudaMalloc((void**)&flag, n * 4) != cudaSuccess ||
-                cudaMalloc((void**)&uidx, (n + 1) * 8) != cudaSuccess ||
-                sb.alloc(n) != SPRS_B200_OK) {
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-            const uint32_t *k1 = nullptr, *p1 = nullptr, *k2 = nullptr, *p2 = nullptr;
-            if ((st = stable_sort_pairs(ctx, sb, d_col, nullptr, n, bits_for(cols), s, &k1, &p1)) !=
-                SPRS_B200_OK)
-                break;
-            gather_u32_kernel<<<grid_for(n), 256, 0, s>>>(d_row, p1, n, row_s);  // row in col order
-            if ((st = stable_sort_pairs(ctx, sb, row_s, p1, n, bits_for(rows), s, &k2, &p2)) !=
-                SPRS_B200_OK)
-                break;
-            gather_u32_kernel<<<grid_for(n), 256, 0, s>>>(d_col, p2, n, col_s);
-            head_flags_kernel<<<grid_for(n), 256, 0, s>>>(k2, col_s, n, flag);
-            ctx->launches += 3;
-            if ((st = device_exclusive_scan<uint32_t, uint64_t>(ctx, flag, n, uidx, s)) != SPRS_B200_OK)
-                break;
-            if (cudaMemcpyAsync(&n_unique, uidx + n, 8, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-                cudaStreamSynchronize(s) != cudaSuccess) {
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-            if (cudaMalloc((void**)&t->d_indices, n_unique * 4 + 16) != cudaSuccess ||
-                cudaMalloc((void**)&t->d_data, n_unique * 8 + 16) != cudaSuccess) {
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-            compress_runs_kernel<<<grid_for(n), 256, 0, s>>>(k2, col_s, p2, flag, uidx, d_val, n,
-                                                            t->d_indices, t->d_data, counts);
-            ctx->launches += 1;
-        } else {
-            if (cudaMalloc((void**)&t->d_indices, 16) != cudaSuccess ||
-                cudaMalloc((void**)&t->d_data, 16) != cudaSuccess) {
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-        }
-        t->nnz = n_unique;
-        if ((st = device_exclusive_scan<uint32_t, uint64_t>(ctx, counts, rows, ip64, s)) != SPRS_B200_OK)
-            break;
-        narrow_kernel<uint64_t, uint32_t><<<grid_for(rows + 1), 256, 0, s>>>(
-            ip64, (uint32_t*)t->d_indptr, rows + 1);
+    SPRS_TRY(counts.alloc(ctx, (rows + 1) * 4, "from_triplets"));
+    SPRS_TRY(ip64.alloc(ctx, (rows + 1) * 8, "from_triplets"));
+    cudaMemsetAsync(counts, 0, (rows + 1) * 4, s);
+    uint64_t n_unique = 0;
+    const uint32_t *k2 = nullptr, *p2 = nullptr;
+    if (n) {
+        SPRS_TRY(row_s.alloc(ctx, n * 4, "from_triplets"));
+        SPRS_TRY(col_s.alloc(ctx, n * 4, "from_triplets"));
+        SPRS_TRY(flag.alloc(ctx, n * 4, "from_triplets"));
+        SPRS_TRY(uidx.alloc(ctx, (n + 1) * 8, "from_triplets"));
+        SPRS_TRY(sb.alloc(ctx, n, "from_triplets"));
+        const uint32_t *k1 = nullptr, *p1 = nullptr;
+        SPRS_TRY(stable_sort_pairs(ctx, sb, d_col, nullptr, n, bits_for(cols), s, &k1, &p1));
+        gather_u32_kernel<<<grid_for(n), 256, 0, s>>>(d_row, p1, n, row_s);  // row in col order
+        SPRS_TRY(stable_sort_pairs(ctx, sb, row_s, p1, n, bits_for(rows), s, &k2, &p2));
+        gather_u32_kernel<<<grid_for(n), 256, 0, s>>>(d_col, p2, n, col_s);
+        head_flags_kernel<<<grid_for(n), 256, 0, s>>>(k2, col_s, n, flag);
+        ctx->launches += 3;
+        SPRS_TRY((device_exclusive_scan<uint32_t, uint64_t>(ctx, flag, n, uidx, s)));
+        SPRS_CUDA(ctx, cudaMemcpyAsync(&n_unique, uidx + n, 8, cudaMemcpyDeviceToHost, s));
+        SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+    }
+    CsmatPtr t = new_result(ctx, SPRS_B200_CSR, rows, cols, n_unique, 4, Arrays::owned);
+    SPRS_TRY(alloc_result(ctx, t.get(), s, "from_triplets"));
+    if (n) {
+        compress_runs_kernel<<<grid_for(n), 256, 0, s>>>(k2, col_s, p2, flag, uidx, d_val, n,
+                                                        t->d_indices, t->d_data, counts);
         ctx->launches += 1;
-    } while (0);
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (st == SPRS_B200_OK && e == cudaSuccess) e = cudaGetLastError();
-    if (st == SPRS_B200_OK && e != cudaSuccess) st = SPRS_B200_ERR_CUDA;
-    if (st == SPRS_B200_ERR_CUDA) sprs_b200_set_error(ctx, "from_triplets: CUDA allocation or kernel failed");
-    if (counts) cudaFree(counts);
-    if (ip64) cudaFree(ip64);
-    if (row_s) cudaFree(row_s);
-    if (col_s) cudaFree(col_s);
-    if (flag) cudaFree(flag);
-    if (uidx) cudaFree(uidx);
-    sb.release();
-    return st;
+    }
+    SPRS_TRY((device_exclusive_scan<uint32_t, uint64_t>(ctx, counts, rows, ip64, s)));
+    narrow_kernel<uint64_t, uint32_t><<<grid_for(rows + 1), 256, 0, s>>>(
+        ip64, (uint32_t*)t->d_indptr, rows + 1);
+    ctx->launches += 1;
+    SPRS_CUDA(ctx, cudaStreamSynchronize(s));
+    SPRS_CUDA(ctx, cudaGetLastError());
+    *out = std::move(t);
+    return SPRS_B200_OK;
 }
 
 // ---- the dense boundary of a sparse matrix: to_dense / assign_to_dense
@@ -685,68 +604,38 @@ int from_dense_run(sprs_b200_ctx* ctx, int storage, uint64_t rows, uint64_t cols
     const uint64_t inner = storage == SPRS_B200_CSR ? cols : rows;
     const uint64_t total = outer * inner;
     const uint64_t n_tiles = (total + DENSE_TILE - 1) / DENSE_TILE;
-    uint32_t* cnt = nullptr;
-    uint64_t* off = nullptr;
-    sprs_b200_csmat* c = nullptr;
-    int st = SPRS_B200_OK;
-    do {
-        uint64_t nnz = 0;
-        if (n_tiles) {
-            if (cudaMallocAsync((void**)&cnt, n_tiles * 4, s) != cudaSuccess ||
-                cudaMallocAsync((void**)&off, (n_tiles + 1) * 8, s) != cudaSuccess) {
-                cudaGetLastError();
-                sprs_b200_set_error(ctx, "from_dense: cudaMallocAsync of the tile counts failed");
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-            from_dense_kernel<false, uint32_t><<<warps_grid(n_tiles), 256, 0, s>>>(
-                m, outer, inner, n_tiles, eps, cnt, nullptr, nullptr, nullptr, nullptr);
-            ctx->launches += 1;
-            if ((st = device_exclusive_scan<uint32_t, uint64_t>(ctx, cnt, n_tiles, off, s)) !=
-                SPRS_B200_OK)
-                break;
-            if (cudaMemcpyAsync(&nnz, off + n_tiles, 8, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-                cudaStreamSynchronize(s) != cudaSuccess) {
-                sprs_b200_set_error(ctx, "from_dense: count pass failed");
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-        }
-        c = new_result(ctx, storage, rows, cols, nnz,
-                       (nnz >= 0xffffffffull || force_indptr64()) ? 8 : 4);
-        if ((st = alloc_result(ctx, c, s)) != SPRS_B200_OK) break;
-        if (n_tiles == 0) {  // no position: indptr is all zeros
-            if (cudaMemsetAsync(c->d_indptr, 0, (outer + 1) * (size_t)c->indptr_bytes, s) !=
-                cudaSuccess) {
-                sprs_b200_set_error(ctx, "from_dense: memset failed");
-                st = SPRS_B200_ERR_CUDA;
-                break;
-            }
-        } else if (c->indptr_bytes == 4) {
-            from_dense_kernel<true, uint32_t><<<warps_grid(n_tiles), 256, 0, s>>>(
-                m, outer, inner, n_tiles, eps, nullptr, off, (uint32_t*)c->d_indptr, c->d_indices,
-                c->d_data);
-        } else {
-            from_dense_kernel<true, uint64_t><<<warps_grid(n_tiles), 256, 0, s>>>(
-                m, outer, inner, n_tiles, eps, nullptr, off, (uint64_t*)c->d_indptr, c->d_indices,
-                c->d_data);
-        }
-        ctx->launches += n_tiles ? 1 : 0;
-        if (cudaGetLastError() != cudaSuccess) {
-            sprs_b200_set_error(ctx, "from_dense: launch failed");
-            st = SPRS_B200_ERR_CUDA;
-            break;
-        }
-        st = finish_result(ctx, c, s, "from_dense");
-    } while (0);
-    if (cnt) cudaFreeAsync(cnt, s);
-    if (off) cudaFreeAsync(off, s);
-    if (st != SPRS_B200_OK) {
-        sprs_b200_csmat_free(c);
-        return st;
+    uint64_t nnz = 0;
+    Owned<uint32_t> cnt;
+    Owned<uint64_t> off;
+    if (n_tiles) {
+        SPRS_TRY(cnt.alloc_async(ctx, n_tiles * 4, s, "from_dense"));
+        SPRS_TRY(off.alloc_async(ctx, (n_tiles + 1) * 8, s, "from_dense"));
+        from_dense_kernel<false, uint32_t><<<warps_grid(n_tiles), 256, 0, s>>>(
+            m, outer, inner, n_tiles, eps, cnt, nullptr, nullptr, nullptr, nullptr);
+        ctx->launches += 1;
+        SPRS_TRY((device_exclusive_scan<uint32_t, uint64_t>(ctx, cnt, n_tiles, off, s)));
+        if (cudaMemcpyAsync(&nnz, off + n_tiles, 8, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+            cudaStreamSynchronize(s) != cudaSuccess)
+            SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "from_dense: count pass failed");
     }
-    *out = c;
-    return SPRS_B200_OK;
+    CsmatPtr c = new_result(ctx, storage, rows, cols, nnz, indptr_bytes_for(nnz), Arrays::pooled);
+    SPRS_TRY(alloc_result(ctx, c.get(), s, "from_dense"));
+    if (n_tiles == 0) {  // no position: indptr is all zeros
+        if (cudaMemsetAsync(c->d_indptr, 0, (outer + 1) * (size_t)c->indptr_bytes, s) != cudaSuccess)
+            SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "from_dense: memset failed");
+    } else if (c->indptr_bytes == 4) {
+        from_dense_kernel<true, uint32_t><<<warps_grid(n_tiles), 256, 0, s>>>(
+            m, outer, inner, n_tiles, eps, nullptr, off, (uint32_t*)c->d_indptr, c->d_indices,
+            c->d_data);
+    } else {
+        from_dense_kernel<true, uint64_t><<<warps_grid(n_tiles), 256, 0, s>>>(
+            m, outer, inner, n_tiles, eps, nullptr, off, (uint64_t*)c->d_indptr, c->d_indices,
+            c->d_data);
+    }
+    ctx->launches += n_tiles ? 1 : 0;
+    if (cudaGetLastError() != cudaSuccess)
+        SPRS_FAIL(ctx, SPRS_B200_ERR_CUDA, "from_dense: launch failed");
+    return finish_result(ctx, c, s, "from_dense", false, out);
 }
 
 // ---- host-buffer plumbing: a strided host view <-> a contiguous outer-major device copy,

@@ -46,15 +46,15 @@
 struct sprs_b200_trisolve {
     sprs_b200_ctx* ctx = nullptr;
     const sprs_b200_csmat* csr = nullptr;  // the rows solved: the mirror (CSR) or own_t (CSC)
-    sprs_b200_csmat* own_t = nullptr;      // CSC mirrors: the device transpose
+    CsmatPtr own_t;                        // CSC mirrors: the device transpose
     int storage = SPRS_B200_CSR, tri = SPRS_B200_TRI_LOWER;
     uint64_t n = 0;
-    uint32_t* d_diag = nullptr;            // per row: offset of the first entry with col >= r
-    uint32_t* d_flags = nullptr;           // per row: epoch of the last solve that finished it
-    unsigned long long* d_words = nullptr; // [0] ticket counter, [1] singular key (plan)
-    unsigned long long* d_progress = nullptr;  // per warp of the solve: rows / heartbeats done
+    Owned<uint32_t> d_diag;                // per row: offset of the first entry with col >= r
+    Owned<uint32_t> d_flags;               // per row: epoch of the last solve that finished it
+    Owned<unsigned long long> d_words;     // [0] ticket counter, [1] singular key (plan)
+    Owned<unsigned long long> d_progress;  // per warp of the solve: rows / heartbeats done
     uint64_t n_progress = 0;               // words in d_progress (warps of the largest grid)
-    unsigned long long* h_err = nullptr;   // mapped pinned word: a wait bound was exceeded
+    Owned<unsigned long long> h_err;       // mapped pinned word: a wait bound was exceeded
     cudaEvent_t ev_last = nullptr;         // recorded behind the last enqueued solve
     uint32_t epoch = 0;
     uint64_t k_ticket = 0;                 // first singular ticket (n: none)
@@ -262,26 +262,21 @@ int singular_status(sprs_b200_trisolve* p) {
 
 void free_plan(sprs_b200_trisolve* p) {
     if (p->ctx) cudaSetDevice(p->ctx->device);
-    if (p->d_diag) cudaFree(p->d_diag);
-    if (p->d_flags) cudaFree(p->d_flags);
-    if (p->d_words) cudaFree(p->d_words);
-    if (p->d_progress) cudaFree(p->d_progress);
-    if (p->h_err) cudaFreeHost(p->h_err);
     if (p->ev_last) cudaEventDestroy(p->ev_last);
-    if (p->own_t) sprs_b200_csmat_free(p->own_t);
     delete p;
 }
+using PlanPtr = std::unique_ptr<sprs_b200_trisolve, FreeWith<free_plan>>;
 
 // the flags, counters and wait-bound words of a plan
 int alloc_solve_state(sprs_b200_trisolve* p, cudaStream_t s) {
     sprs_b200_ctx* ctx = p->ctx;
     const uint64_t n = p->n;
-    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_flags, n * sizeof(uint32_t) + 16));
-    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_words, 2 * sizeof(unsigned long long)));
+    SPRS_TRY(p->d_flags.alloc(ctx, n * sizeof(uint32_t) + 16, "trisolve"));
+    SPRS_TRY(p->d_words.alloc(ctx, 2 * sizeof(unsigned long long), "trisolve"));
     p->n_progress = (uint64_t)ctx->sm_count * TRI_CTAS_PER_SM * (TRI_THREADS / 32);
-    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_progress, p->n_progress * sizeof(unsigned long long)));
+    SPRS_TRY(p->d_progress.alloc(ctx, p->n_progress * sizeof(unsigned long long), "trisolve"));
     SPRS_CUDA(ctx, cudaEventCreateWithFlags(&p->ev_last, cudaEventDisableTiming));
-    SPRS_CUDA(ctx, cudaMallocHost((void**)&p->h_err, sizeof(unsigned long long)));
+    SPRS_TRY(p->h_err.alloc_pinned(ctx, sizeof(unsigned long long), "trisolve"));
     *p->h_err = 0;
     SPRS_CUDA(ctx, cudaMemsetAsync(p->d_flags, 0, n * sizeof(uint32_t) + 16, s));
     return SPRS_B200_OK;
@@ -291,14 +286,13 @@ int build_plan(sprs_b200_trisolve* p, const sprs_b200_csmat* mat) {
     sprs_b200_ctx* ctx = p->ctx;
     cudaStream_t s = ctx->stream;
     if (mat->storage == SPRS_B200_CSC) {
-        p->own_t = new sprs_b200_csmat();
-        SPRS_TRY(transpose_launch(ctx, mat, p->own_t, s));
-        p->csr = p->own_t;
+        SPRS_TRY(transpose_launch(ctx, mat, &p->own_t, s));
+        p->csr = p->own_t.get();
     } else {
         p->csr = mat;
     }
     const uint64_t n = p->n;
-    SPRS_CUDA(ctx, cudaMalloc((void**)&p->d_diag, n * sizeof(uint32_t) + 16));
+    SPRS_TRY(p->d_diag.alloc(ctx, n * sizeof(uint32_t) + 16, "trisolve"));
     SPRS_TRY(alloc_solve_state(p, s));
     unsigned long long key = ~0ull;
     SPRS_CUDA(ctx, cudaMemcpyAsync(p->d_words + 1, &key, sizeof(key), cudaMemcpyHostToDevice, s));
@@ -324,19 +318,15 @@ int build_plan(sprs_b200_trisolve* p, const sprs_b200_csmat* mat) {
 int trisolve_unit_plan(sprs_b200_ctx* ctx, const sprs_b200_csmat* csr, int tri,
                        sprs_b200_trisolve** out) {
     *out = nullptr;
-    auto* p = new sprs_b200_trisolve();
+    PlanPtr p(new sprs_b200_trisolve());
     p->ctx = ctx;
     p->csr = csr;
     p->tri = tri;
     p->n = csr->rows;
     p->k_ticket = p->n;
     p->unit = true;
-    const int st = alloc_solve_state(p, ctx->stream);
-    if (st != SPRS_B200_OK) {
-        free_plan(p);
-        return st;
-    }
-    *out = p;
+    SPRS_TRY(alloc_solve_state(p.get(), ctx->stream));
+    *out = p.release();
     return SPRS_B200_OK;
 }
 
@@ -359,17 +349,13 @@ int sprs_b200_trisolve_plan(sprs_b200_ctx* ctx, const sprs_b200_csmat* mat, int 
     if (mat->rows != mat->cols)
         SPRS_FAIL(ctx, SPRS_B200_ERR_DIMENSION, "Non square matrix passed to solver");
     SPRS_CUDA(ctx, cudaSetDevice(ctx->device));
-    auto* p = new sprs_b200_trisolve();
+    PlanPtr p(new sprs_b200_trisolve());
     p->ctx = ctx;
     p->storage = mat->storage;
     p->tri = tri;
     p->n = mat->rows;
-    const int st = build_plan(p, mat);
-    if (st != SPRS_B200_OK) {
-        free_plan(p);
-        return st;
-    }
-    *out = p;
+    SPRS_TRY(build_plan(p.get(), mat));
+    *out = p.release();
     return SPRS_B200_OK;
 }
 
