@@ -5,12 +5,20 @@ assembling CSR from candidate keys; the keys and values come from the counter-ba
 kernels in csrc/gen.cu so that every rank regenerates identical matrices.
 
   rand_csr(...)   sprs-rand's distribution (sprs-rand/src/lib.rs:24-81): nnz =
-                  ceil(density * rows * cols), a uniform random row per non-zero,
-                  distinct uniform columns per row, values N(0,1) (lib.rs:85-88).
+                  ceil(density * rows * cols) exactly, a uniform random row per non-zero,
+                  distinct uniform columns per row, values N(0,1) (lib.rs:85-88).  Uniform
+                  cells are drawn, duplicates dropped, and more drawn until at least the
+                  target are distinct, then thinned by hash to the target; ValueError when
+                  the target exceeds rows * cols (the reference asserts density <= 1).
   rmat_csr(...)   this repo's R-MAT definition (the reference has none, SURVEY F8):
                   Graph500 (a,b,c,d) = (0.57,0.19,0.19,0.05), scale = ceil(log2 n),
                   candidates with an index >= n rejected, duplicates dropped, then
-                  thinned uniformly to ~target nnz.
+                  thinned uniformly to the target nnz (exactly when at most 2^27 keys are
+                  distinct, to within sampling noise of it otherwise); ValueError when
+                  six oversampling passes leave fewer distinct keys than the target.
+
+tests/gen_model.py restates all of it on the host; tests/test_gpu_gen_bits.py compares the two
+bit for bit and pins the benchmark matrices by digest.
 """
 import ctypes as C
 import math
@@ -141,12 +149,17 @@ def _collect(ctx, gen, n_candidates, chunk=1 << 27):
 def rand_csr(ctx, rows, cols, nnz_per_row, seed=0x5EED0002):
     """sprs-rand semantics; exact nnz = ceil(density*rows*cols) (lib.rs:37-38)."""
     target = int(math.ceil(nnz_per_row * rows))
+    if target > rows * cols:
+        raise ValueError("rand_csr: %d non-zeros do not fit %d x %d" % (target, rows, cols))
     over = target + max(4096, target // 512)
 
     def gen(first, cnt, out):
         ctx.check(ctx.lib.sprs_b200_gen_uniform_keys(ctx.h, seed, rows, cols, first, cnt,
                                                      _dptr(out), _stream_ptr()))
     keys = _collect(ctx, gen, over)
+    while keys.numel() < target:  # dense targets: duplicates ate the slack of the first pass
+        over = int(over * 1.5)
+        keys = _collect(ctx, gen, over)
     keys = _thin(ctx, keys, target, seed, exact=True)
     return _keys_to_csr(ctx, keys, rows, cols, seed)
 
@@ -166,6 +179,9 @@ def rmat_csr(ctx, n, nnz_per_row, seed=0x5EED0005, abc=(0.57, 0.19, 0.19), overs
         if keys.numel() >= target:
             break
         factor *= 1.5
+    else:
+        raise ValueError("rmat_csr: %d distinct keys of the %d asked for after six passes"
+                         % (keys.numel(), target))
     keys = _thin(ctx, keys, target, seed, exact=keys.numel() <= (1 << 27))
     return _keys_to_csr(ctx, keys, n, n, seed)
 
